@@ -84,6 +84,7 @@ struct rafting_engine {
     struct rafting::SegLog* seglog = nullptr;   // HBM entry buffer (seglog.cuh), created by rafting_log_config
     cudaEvent_t ev_seg = nullptr;
     uint64_t launches = 0, events = 0;
+    bool follows_step = false;         // the launch being made directly follows a step kernel of the same sequence on its stream
     uint32_t lease_counter = 0;
     uint32_t* d_perm = nullptr;        // [NCLS * G] class-sorted positions of the step being launched (classify_kernel)
     uint32_t* d_perm_cnt = nullptr;    // class sizes
@@ -311,7 +312,15 @@ static int launch_pair(rafting_engine* e, const InboxD& in0, const OutboxD& out,
     if (in0.perm) return fail(RAFTING_E_INVAL, "launch_pair: pair_kernel takes only steps launched without a class sort");
     if (in0.n == 0) return RAFTING_OK;
     const uint32_t blocks = (in0.n + TPB - 1) / TPB;
-    pair::pair_kernel<NSTP><<<blocks, pair::PTPB, smem, st>>>(e->T, in0, out, e->d_cfg, e->dcfg);
+    // Directly behind the previous step's kernel, the launch is programmatic (Hopper PDL): its blocks take the SMs the
+    // previous launch's blocks free, and stage their first inbox rows while its last blocks finish; griddepcontrol.wait
+    // holds every table / outbox access until the previous grid has completed and its writes are visible.
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = dim3(blocks); lc.blockDim = dim3(pair::PTPB); lc.dynamicSmemBytes = smem; lc.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
+    lc.attrs = at; lc.numAttrs = e->follows_step ? 1u : 0u;
+    CU(cudaLaunchKernelEx(&lc, pair::pair_kernel<NSTP>, e->T, in0, out, (const CfgD*)e->d_cfg, e->dcfg));
     return RAFTING_OK;
 }
 static int launch_looped(rafting_engine* e, const InboxD& in, const OutboxD& out, cudaStream_t st) {
@@ -395,7 +404,11 @@ extern "C" int rafting_step_device_seq(rafting_engine_t* e, const rafting_inbox_
     if (!e || !ins || !outs) return fail(RAFTING_E_INVAL, "null argument");
     if (gather && stream && (cudaStream_t)stream != e->stream) return fail(RAFTING_E_INVAL, "gathers follow the engine's own stream");
     for (uint32_t k = 0; k < n; k++) {
-        int rc = rafting_step_device(e, &ins[k], &outs[k], stream); if (rc) return rc;
+        // without gathers, launch k's only predecessor on the stream is launch k-1's step kernel: none of them writes an inbox
+        e->follows_step = k > 0 && !gather;
+        int rc = rafting_step_device(e, &ins[k], &outs[k], stream);
+        e->follows_step = false;
+        if (rc) return rc;
         if (gather) { rc = rafting_allgather_commit_from(e, outs[k].commit_index, nullptr, nullptr); if (rc) return rc; }
     }
     return RAFTING_OK;

@@ -57,6 +57,8 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
     __shared__ KArgs ka;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     PStage* stage = reinterpret_cast<PStage*>(smem_raw);
+    // a programmatic launch behind this one (launch_pair) may start its blocks as soon as these exit
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (threadIdx.x == 0) { ka.T = T; ka.in = in; ka.out = out; ka.cfg = cfgp; }
     __syncthreads();
     const uint32_t tid = threadIdx.x, f = tid & 1u, tl = tid >> 1;       // follower lane, group slot in the block
@@ -68,12 +70,7 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
     uint32_t gid = valid ? (in.gids ? in.gids[i] : i) : 0u;
     if (gid >= T.G) { valid = false; gid = 0; }
     // every thread of a warp stays in the row loop (full-mask shuffles); an invalid pair computes on group 0 and stores nothing
-
-    GS g; LS x;
-    load_hot(T, gid, g); g.dirty = 0; g.electTerm = 0; g.electInc = 0; g.votes = 0;
-    if (!valid) g.word = 0;
     const size_t li = (size_t)gid * 2u + f;
-    load_lane(T, li, x);
     const bool hasOps = in.op_meta != nullptr, hasEv = in.ev_meta != nullptr, hasAb = in.op_ab != nullptr, hasEl = in.ev_el != nullptr;
 
 #define PAIR_ISSUE(R_)                                                                                          \
@@ -97,6 +94,13 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
     }
 #pragma unroll
     for (int p = 0; p < NST - 1; p++) PAIR_ISSUE((uint32_t)p);
+    // the inbox is read-only here and written by no step kernel; the tables and the outbox are the previous launch's: wait
+    // for it (a no-op unless this is a programmatic launch)
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    GS g; LS x;
+    load_hot(T, gid, g); g.dirty = 0; g.electTerm = 0; g.electInc = 0; g.votes = 0;
+    if (!valid) g.word = 0;
+    load_lane(T, li, x);
 
     const uint32_t lane = threadIdx.x & 31u;
     for (uint32_t r = 0; r < in.rows; r++) {
@@ -137,7 +141,8 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
             }
             // replicateLog for my follower: which branch (Leader.java:156-217), decided before anything changes
             const int64_t hiNew = (submit && ready) ? g.hi + (int64_t)count : g.hi;
-            const int limit = RAFTING_IN_FLIGHT_LIMIT / (hb ? 10 : 1), fetch = RAFTING_REPLICATE_LIMIT >> (hb ? 1 : 0);
+            // two constants, not a division by a runtime value: the division is a subroutine CALL on the row's chain
+            const int limit = hb ? RAFTING_IN_FLIGHT_LIMIT / 10 : RAFTING_IN_FLIGHT_LIMIT, fetch = RAFTING_REPLICATE_LIMIT >> (hb ? 1 : 0);
             const int64_t p = (int64_t)((uint64_t)x.next - 1u);
             int cls;                                                    // 4 unavailable, 3 in-flight limit, 2 snapshot, 1 entries, 0 general
             if (unav) cls = 4;
