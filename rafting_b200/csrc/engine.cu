@@ -277,30 +277,19 @@ extern "C" int rafting_group_close(rafting_engine_t* e, uint32_t gid) {
 // R<=5 -> <4,3>, R<=9 -> <8,2>, larger clusters keep their slots in local memory and read the inbox directly
 template <int FT, int NST>
 static int launch_t(rafting_engine* e, const InboxD& in, const OutboxD& out, cudaStream_t st) {
-    const size_t smem = NST > 0 ? (size_t)NST * sizeof(Stage<FT>) + (size_t)NST * (TPB / 32) * 8 + 16 : 0;
+    const size_t smem = (size_t)NST * sizeof(Stage<FT>);
     static bool configured[64] = {false};
     if (smem > 0 && !configured[e->cfg.device & 63]) {
-        CU(cudaFuncSetAttribute(unrolled::step_kernel<FT, NST, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (NST > 0) CU(cudaFuncSetAttribute(unrolled::step_kernel<FT, (NST > 0 ? NST : 1), true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CU(cudaFuncSetAttribute(unrolled::step_kernel<FT, NST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured[e->cfg.device & 63] = true;
     }
-    const uint32_t blocks = (in.n + TPB - 1) / TPB + (in.perm ? (uint32_t)NCLS : 0u), full = in.n / TPB;   // + NCLS: every class is padded to a block
+    const uint32_t blocks = (in.n + TPB - 1) / TPB + (in.perm ? (uint32_t)NCLS : 0u);   // + NCLS: every class is padded to a block
     if (in.n == 0) return RAFTING_OK;
-    // TMA bulk staging needs full blocks, F == FT and 16-byte aligned column slices on every row
-    auto al16 = [](const void* p) { return ((uintptr_t)p & 15u) == 0; };
-    const bool bulk = NST > 0 && !in.perm && e->F == (uint32_t)FT && full > 0 && (in.n % 2 == 0 || in.rows == 1) &&
-                      al16(in.op_meta) && al16(in.op_nr) && al16(in.op_ab) && al16(in.ev_meta) && al16(in.ev_tn) && al16(in.ev_el) &&
-                      getenv("RAFTING_BULK_STAGING") != nullptr;   // opt-in: measured slower than per-thread cp.async (DESIGN.md §5)
-    if (bulk) {
-        unrolled::step_kernel<FT, (NST > 0 ? NST : 1), true><<<full, TPB, smem, st>>>(e->T, in, out, e->d_cfg, e->dcfg, 0u);
-        if (blocks > full) unrolled::step_kernel<FT, NST, false><<<blocks - full, TPB, smem, st>>>(e->T, in, out, e->d_cfg, e->dcfg, full);
-    } else {
-        unrolled::step_kernel<FT, NST, false><<<blocks, TPB, smem, st>>>(e->T, in, out, e->d_cfg, e->dcfg, 0u);
-    }
+    unrolled::step_kernel<FT, NST><<<blocks, TPB, smem, st>>>(e->T, in, out, e->d_cfg, e->dcfg);
     return RAFTING_OK;
 }
 // R = 3, a step launched without a class sort (the leader stream): one thread per (group, follower) (pair_kernel.cuh, v7),
-// which measured faster than the thread-per-group kernel (v6) on an H100 (DESIGN.md §5); RAFTING_NO_PAIR=1 selects v6
+// which measured faster than the thread-per-group kernel (v6) on an H100 (DESIGN.md §5)
 static int launch_pair(rafting_engine* e, const InboxD& in0, const OutboxD& out, cudaStream_t st) {
     constexpr int NSTP = 3;
     const size_t smem = (size_t)NSTP * sizeof(pair::PStage);
@@ -326,7 +315,7 @@ static int launch_pair(rafting_engine* e, const InboxD& in0, const OutboxD& out,
 static int launch_looped(rafting_engine* e, const InboxD& in, const OutboxD& out, cudaStream_t st) {
     const uint32_t blocks = (in.n + TPB - 1) / TPB;
     if (blocks == 0) return RAFTING_OK;
-    looped::step_kernel<32, 0, false><<<blocks, TPB, 64, st>>>(e->T, in, out, e->d_cfg, e->dcfg, 0u);
+    looped::step_kernel<32, 0><<<blocks, TPB, 0, st>>>(e->T, in, out, e->d_cfg, e->dcfg);
     return RAFTING_OK;
 }
 static int launch_step(rafting_engine* e, const InboxD& in0, const OutboxD& out, cudaStream_t st) {
@@ -336,26 +325,16 @@ static int launch_step(rafting_engine* e, const InboxD& in0, const OutboxD& out,
     InboxD in = in0; in.perm = nullptr; in.perm_cnt = nullptr;
     // A step that may hold inbound requests mixes steady-state leaders with groups that need the generic handlers;
     // one slow lane stalls its whole warp, so such steps are launched class-sorted (DESIGN.md §5)
-    static const bool sortOff = getenv("RAFTING_NO_CLASS_SORT") != nullptr;
-    if (!(in.flags & RAFTING_INBOX_NO_REQUESTS) && in.op_meta && in.n >= 2048 && F <= 8 && !sortOff) {
+    if (!(in.flags & RAFTING_INBOX_NO_REQUESTS) && in.op_meta && in.n >= 2048 && F <= 8) {
         CU(cudaMemsetAsync(e->d_perm_cnt, 0, NCLS * 4, st));
         classify_kernel<<<(in.n + 255) / 256, 256, 0, st>>>(e->T, in, e->d_perm, e->d_perm_cnt);
         in.perm = e->d_perm; in.perm_cnt = e->d_perm_cnt;
     }
-    // slow classes in their own kernel with their own register cap (RAFTING_SLOW_KERNEL=0 keeps them inside step_kernel;
-    // =2 / =3 pick the other caps compiled in for A/B runs)
-    static const int slowVar = getenv("RAFTING_SLOW_KERNEL") ? atoi(getenv("RAFTING_SLOW_KERNEL")) : 1;
-    if (in.perm && slowVar > 0 && (F == 2 || (F > 2 && F <= 4))) {
+    // at F = 2..4 the slow classes run in a kernel of their own, with their own register cap
+    if (in.perm && F >= 2 && F <= 4) {
         const uint32_t sb = (in.n + unrolled::SLOW_TPB - 1) / unrolled::SLOW_TPB + (uint32_t)NCLS;
-        if (F == 2) {
-            if (slowVar == 2) unrolled::slow_kernel<2, 6><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
-            else if (slowVar == 3) unrolled::slow_kernel<2, 8><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
-            else unrolled::slow_kernel<2, 4><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
-        } else {
-            if (slowVar == 2) unrolled::slow_kernel<4, 6><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
-            else if (slowVar == 3) unrolled::slow_kernel<4, 8><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
-            else unrolled::slow_kernel<4, 4><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
-        }
+        if (F == 2) unrolled::slow_kernel<2, 4><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
+        else unrolled::slow_kernel<4, 4><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
         in.flags |= INBOX_INTERNAL_SLOW_ELSEWHERE;
     }
     if (F == 1) rc = launch_t<1, 3>(e, in, out, st);
@@ -365,8 +344,7 @@ static int launch_step(rafting_engine* e, const InboxD& in0, const OutboxD& out,
     else if (F == 2) {
         // v7 (pair_kernel.cuh) measured faster than v6 on the leader stream on an H100 and slower on class-sorted steps
         // (config #5), same-call A/Bs (DESIGN.md §5): it runs the steps launched without a class sort
-        static const bool pairOn = getenv("RAFTING_NO_PAIR") == nullptr;
-        rc = pairOn && !in.perm ? launch_pair(e, in, out, st) : launch_t<2, RAFTING_NST2>(e, in, out, st);
+        rc = !in.perm ? launch_pair(e, in, out, st) : launch_t<2, RAFTING_NST2>(e, in, out, st);
     }
     else if (F <= 4) rc = launch_t<4, 3>(e, in, out, st);
     else if (F <= 8) rc = launch_t<8, 2>(e, in, out, st);

@@ -75,3 +75,12 @@ def test_product_does_not_touch_the_oracle():
                 assert "oracle/" not in txt.replace("nothing here includes or links oracle/", "").replace(
                     "Nothing here includes or links oracle/", "") or f in ("engine.cu",), f
                 assert "import oracle" not in txt and "from oracle" not in txt, f
+
+
+def test_native_code_reads_no_environment_switches():
+    """What a step launches depends on its inputs and the engine's configuration only, never on the process environment."""
+    csrc = os.path.join(ROOT, "rafting_b200", "csrc")
+    for dirpath, _, files in os.walk(csrc):
+        for f in files:
+            if f.endswith((".cu", ".cuh", ".inc", ".cpp")):
+                assert "getenv" not in open(os.path.join(dirpath, f), errors="replace").read(), f

@@ -64,19 +64,6 @@ def test_leader_stream_parity(engine_mod, R, G, rows):
     assert len(set(d.tolist())) > 1
 
 
-def test_leader_stream_parity_with_the_thread_per_group_kernel():
-    """At R = 3 the leader stream runs pair_kernel; RAFTING_NO_PAIR=1 (read once per process) selects the thread-per-group
-    step kernel instead.  The same parity cases, a full and a partial last block, in a process of their own with it set."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    ids = [f"tests/test_engine_gpu.py::test_leader_stream_parity[{c}]" for c in ("3-4096-8", "3-777-5")]
-    res = subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", *ids], capture_output=True, text=True,
-                         timeout=600, env=dict(os.environ, RAFTING_NO_PAIR="1"), cwd=root)
-    assert res.returncode == 0 and "2 passed" in res.stdout, (res.stdout[-2000:], res.stderr[-2000:])
-
-
 @pytest.mark.parametrize("R,local_slot,pre_vote,seed", [(3, 0, True, 1), (3, 2, False, 2), (5, 2, True, 3), (4, 1, True, 4), (7, 6, False, 5)])
 def test_fuzz_parity_all_event_kinds(engine_mod, R, local_slot, pre_vote, seed):
     """Random mix of every op and lane-event kind (requests, votes, snapshots, flushes, acks, forged

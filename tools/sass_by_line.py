@@ -56,7 +56,7 @@ def main():
     ncu_csv, sass, ksub = sys.argv[1:4]
     which = int(sys.argv[4]) if len(sys.argv) > 4 else -1
     top = int(sys.argv[5]) if len(sys.argv) > 5 else 40
-    mangled = {"pair_kernel": "pair11pair_kernel", "step_kernel<(int)2, (int)3, (bool)0>": "unrolled11step_kernelILi2ELi3ELb0"}.get(ksub, ksub)
+    mangled = {"pair_kernel": "pair11pair_kernel", "step_kernel<(int)2, (int)3>": "unrolled11step_kernelILi2ELi3E"}.get(ksub, ksub)
     inst = load_ncu(ncu_csv, ksub, which)
     lines = load_lines(sass, mangled)
     per = collections.defaultdict(lambda: [0, 0, 0.0])
