@@ -414,8 +414,10 @@ int rafting_step_wait_slot (rafting_engine_t* e, uint32_t slot);
  *   * the (epochAtSend, lastIndexAtSend) echo stays in an HBM in-flight table: pack gives every AE / IS plan a TAG (a free
  *     slot 0..31 of its (group, follower) lane), the reply echoes the tag, unpack looks the pair up and frees the slot.
  *     No free slot (more than 32 RPCs of one lane outstanding): tag 255, and the reply must come back as an escape record.
- *   * dense steps only (no active list), no inbound-request ops (RAFTING_INBOX_NO_REQUESTS is implied): SUBMIT / TIMEOUT
- *     ops, AE / IS acks; vote replies and anything irregular use the escape list.
+ *   * dense steps only (no active list).  op_c carries SUBMIT / TIMEOUT ops, ev_c AE / IS acks; vote replies and anything
+ *     irregular use the escape lists.  Inbound requests ride beside the inbox in a request list (rafting_creqs_t, below):
+ *     AppendEntries as 32-byte records, every other request kind as an op escape.  A step without requests runs as
+ *     RAFTING_INBOX_NO_REQUESTS.
  *   * wire words are 32 bits: 4 B per lane slot + 4 B per group row up, 4 B per lane slot + 1 B per group row down.
  *   * a tag is freed by the compact reply that echoes it (every RPC completes exactly once: reply, error or cancellation,
  *     Async.java:239-254).  Dense and compact steps can be mixed slot by slot, but the reply to a compact-planned RPC should come
@@ -457,8 +459,10 @@ typedef struct rafting_cinbox {
  *              leaderCommit = commit_index[g] - dcommit, epochAtSend = epoch[g].x          (dprev < 256, dcommit < 128)
  *          IS  (epoch.index, epoch.term) = epoch[g], leaderCommit as above
  *          SKIP_INFLIGHT / UNAVAILABLE: no payload
- * rep_c  : per-event error code of the row's group op (rafting_outbox_t.rep_meta bits 8..15); a row whose op produced a
- *          REPLY (inbound requests are not part of compact steps, but the generic handler may answer) is escaped         */
+ * rep_c  : bits 0..5 per-event error code of the row's group op (rafting_outbox_t.rep_meta bits 8..15) | 6 success |
+ *          7 compact reply: a valid reply whose RaftResponse.term() equals current_term[g] at the end of the step.
+ *          Bits 6 and 7 are set only by steps begun with a request list (rafting_step_begin_compact_req with reqs != NULL);
+ *          every other valid reply travels as a RAFTING_CESC_REPLY escape record                                         */
 #define RAFTING_CPLAN_KIND(w)    ((uint32_t)(w) & 7u)
 #define RAFTING_CPLAN_HB(w)      (((uint32_t)(w) >> 3) & 1u)
 #define RAFTING_CPLAN_ESCAPED(w) (((uint32_t)(w) >> 4) & 1u)
@@ -492,6 +496,60 @@ int rafting_compact_layout(uint32_t rows, uint32_t max_groups, uint32_t follower
                            uint64_t in_off[6], uint64_t out_off[12]);
 int rafting_step_begin_compact(rafting_engine_t* e, uint32_t slot /* 0..3 */, const rafting_cinbox_t* in_host,
                                const rafting_coutbox_t* out_host);
+/* Inbound requests of a compact step.  Every slot (row * G + gid) takes at most ONE group op: a non-NONE op_c word, a
+ * record or an op escape.
+ * rafting_creq_t: one inbound AppendEntries in 32 bytes.  It fits when
+ *          the election-timeout draw is 0, op_e == prevLogIndex + 1, every entry term equals the request's term,
+ *          0 <= term - prevLogTerm < 2^32, leaderCommit - prevLogIndex fits an int32, 0 <= now - row_base[row] <= 65535,
+ *          count <= 63 and the peer slot < 32.
+ *        meta bits 0..4 peer slot | 5..10 entry count | 11..15 zero (else malformed) | 16..31 now - row_base[row] (ms, unsigned)
+ *        The step sees: kind AE, a = term, b = prev_index, c = term - d_prev_term, d = prev_index + d_commit,
+ *        e = prev_index + 1, and `count` entries of term `term`, which the engine writes into the entry pool itself.
+ *        Every field is relative to the request itself or to row_base, never to engine state: a pump encodes a step while
+ *        earlier ones are still in flight.
+ * rafting_cesc_op_t: any other request (PreVote / RequestVote / InstallSnapshot / FLUSH, an AppendEntries that breaks a
+ *        rule above) or a SUBMIT / TIMEOUT with an explicit draw, in full.  Its entry terms sit at ent_terms[ent ...].
+ * Both lists are strictly increasing in slot; slots >= rows * G are ignored.  A slot claimed twice (an op_c word and a
+ * record or op escape, a record and an op escape, the same slot twice in one list) is answered with RAFTING_ERR_BAD_EVENT:
+ * unpack gives it the op kind RAFTING_COP_MALFORMED with now = row_base[row] and every other field 0.  A list that
+ * decreases anywhere makes every op of both lists malformed.
+ * Entry pool of the step: ent_terms[0 .. ent_count) then the records' terms in list order, req_entries in all;
+ * ent_count + req_entries > cfg.entry_pool_cap is RAFTING_E_CAPACITY.  A record whose entries would end past the pool gets
+ * an entry offset past it, so the step answers it with RAFTING_ERR_BAD_EVENT.                                          */
+#define RAFTING_CREQ_MAKE(peer, count, dt) \
+    ((uint32_t)((peer) & 0x1fu) | ((uint32_t)((count) & 0x3fu) << 5) | ((uint32_t)((dt) & 0xffffu) << 16))
+#define RAFTING_CREQ_PEER(m)  ((uint32_t)(m) & 0x1fu)
+#define RAFTING_CREQ_COUNT(m) (((uint32_t)(m) >> 5) & 0x3fu)
+#define RAFTING_CREQ_DT(m)    ((uint32_t)(m) >> 16)
+#define RAFTING_COP_MALFORMED 0xffu
+typedef struct rafting_creq {
+    uint32_t slot;                   /* row * G + gid */
+    uint32_t meta;                   /* RAFTING_CREQ_MAKE(peer, count, now - row_base[row]) */
+    int64_t  term;                   /* the RPC's term; every entry of the request carries it */
+    int64_t  prev_index;             /* prevLogIndex */
+    uint32_t d_prev_term;            /* term - prevLogTerm */
+    int32_t  d_commit;               /* leaderCommit - prevLogIndex */
+} rafting_creq_t;
+typedef struct rafting_cesc_op {
+    uint32_t slot, ent;              /* row * G + gid; offset of its entry terms in ent_terms */
+    uint64_t op_meta;                /* lo32 RAFTING_OP_MAKE(kind, peer, count); hi32 ignored */
+    int64_t  now_ms, draw, a, b, c, d, e;
+} rafting_cesc_op_t;
+typedef struct rafting_creqs {
+    uint32_t n_req, n_op_esc;
+    const rafting_creq_t*    req;       /* [n_req] */
+    const rafting_cesc_op_t* op_esc;    /* [n_op_esc] */
+    const int64_t*           ent_terms; /* [ent_count] entry terms of the escaped AppendEntries */
+    uint32_t ent_count;
+    uint32_t req_entries;               /* sum of the records' counts */
+} rafting_creqs_t;
+/* Byte offsets of req, op_esc and ent_terms inside ONE pinned block, and its size: carved this way the request list goes
+   up in one copy (none when both lists are empty).  off: req, op_esc, ent_terms, total */
+int rafting_compact_req_layout(uint32_t n_req, uint32_t n_op_esc, uint32_t ent_count, uint64_t off[4]);
+/* rafting_step_begin_compact with a request list.  reqs == NULL is exactly rafting_step_begin_compact; with a list (even
+   an empty one) rep_c carries compact replies.  rafting_step_wait_compact / rafting_step_fetch_dense serve both. */
+int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot /* 0..3 */, const rafting_cinbox_t* in_host,
+                                   const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host);
 int rafting_step_wait_compact (rafting_engine_t* e, uint32_t slot);
 /* the dense outbox of the compact step last waited for in `slot` (every column that is non-NULL in out_host): the lossless
    fallback when the escape list overflowed */

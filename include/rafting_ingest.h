@@ -186,6 +186,20 @@ int rafting_request_to_inbox(const rafting_req_rec_t* r, const int64_t* entry_te
 int rafting_outbox_to_replies(const rafting_outbox_t* ob, uint32_t n_groups, uint32_t local_slot, const rafting_req_rec_t* placed,
                               const uint8_t* placed_row, uint32_t n, rafting_batch_rec_t* out, uint32_t* n_out);
 
+/* The same two ends for the compact host path (include/rafting_b200.h, rafting_step_begin_compact_req).
+ * rafting_request_to_creq places one record at (row, gid) of a compact step: an AppendEntries that fits the record rules
+ * becomes a rafting_creq_t (its time relative to in->row_base[row], which the caller sets before placing), anything else a
+ * rafting_cesc_op_t whose entry terms are appended to q->ent_terms.  Both lists stay strictly increasing (placing in slot
+ * order appends).  The list arrays are the caller's, with room for req_cap / esc_cap / ent_cap entries; q's counts grow.
+ * RAFTING_E_INVAL: slot taken (an op_c word, a record or an op escape), gid / row out of range, no room. */
+int rafting_request_to_creq(const rafting_req_rec_t* r, const int64_t* entry_terms, uint32_t row, int64_t now_ms, int host_result,
+                            const rafting_cinbox_t* in, uint32_t n_groups, rafting_creqs_t* q, uint32_t req_cap, uint32_t esc_cap,
+                            uint32_t ent_cap);
+/* rafting_outbox_to_replies over a waited-for compact outbox: the reply of a placed request is its rep_c byte (bit 7) or its
+ * RAFTING_CESC_REPLY escape record.  RAFTING_E_CAPACITY when the escape list overflowed (fetch the dense outbox instead). */
+int rafting_coutbox_to_replies(const rafting_coutbox_t* co, uint32_t n_groups, uint32_t local_slot, const rafting_req_rec_t* placed,
+                               const uint8_t* placed_row, uint32_t n, rafting_batch_rec_t* out, uint32_t* n_out);
+
 /* ---- replies -> compact wire words (the compact host path of include/rafting_b200.h) -------------------------------------
  * The pending-invocation table of the pump: what NettyNode keeps per connection as (scope, sequence) -> Invocation
  * (NettyNode.java:88-90, Async.java) — here (peer, sequence) -> the group, the follower lane, the TAG the plan was sent under

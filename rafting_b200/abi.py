@@ -344,6 +344,22 @@ class CInboxC(C.Structure):
                 ("row_base", C.c_void_p), ("op_c", C.c_void_p), ("op_unavail", C.c_void_p), ("ev_c", C.c_void_p), ("esc", C.c_void_p)]
 
 
+COP_MALFORMED = 0xFF                                  # op kind of a slot claimed twice in a compact step
+CREQ = np.dtype([("slot", "<u4"), ("meta", "<u4"), ("term", "<i8"), ("prev_index", "<i8"), ("d_prev_term", "<u4"), ("d_commit", "<i4")])
+CESC_OP = np.dtype([("slot", "<u4"), ("ent", "<u4"), ("op_meta", "<u8"), ("now_ms", "<i8"), ("draw", "<i8"), ("a", "<i8"), ("b", "<i8"),
+                    ("c", "<i8"), ("d", "<i8"), ("e", "<i8")])
+assert CREQ.itemsize == 32 and CESC_OP.itemsize == 72
+
+
+def creq_make(peer: int, count: int, dt: int) -> int:
+    return (peer & 0x1F) | ((count & 0x3F) << 5) | ((dt & 0xFFFF) << 16)
+
+
+class CReqsC(C.Structure):
+    _fields_ = [("n_req", C.c_uint32), ("n_op_esc", C.c_uint32), ("req", C.c_void_p), ("op_esc", C.c_void_p),
+                ("ent_terms", C.c_void_p), ("ent_count", C.c_uint32), ("req_entries", C.c_uint32)]
+
+
 class COutboxC(C.Structure):
     _fields_ = [("plan_c", C.c_void_p), ("rep_c", C.c_void_p),
                 ("commit_index", C.c_void_p), ("current_term", C.c_void_p), ("role_word", C.c_void_p), ("incarnation", C.c_void_p),

@@ -2,6 +2,7 @@
 with the engine — numpy only.
 
   encode_inbox   dense lane events / group ops  ->  ev_c / op_c / row_base (+ escape records for whatever breaks a compact rule)
+                 and, for steps with inbound requests, the request list (AppendEntries records + op escapes)
   decode_outbox  plan_c / rep_c / group columns / escape records  ->  the dense outbox columns
 
 The engine's own unpack / pack kernels (rafting_b200/csrc/compact.cuh) are the inverse of these two; tests/test_compact_gpu.py
@@ -36,6 +37,28 @@ class CompactInbox:
         c.op_unavail = None if self.op_unavail is None else self.op_unavail.ctypes.data
         c.ev_c = None if self.ev_c is None else self.ev_c.ctypes.data
         c.esc = self.esc.ctypes.data if len(self.esc) else None
+        return c
+
+
+class CompactRequests:
+    """Inbound requests of a compact step (rafting_creqs_t): AppendEntries records, op escapes and the escapes' entry terms."""
+
+    def __init__(self, req=None, op_esc=None, ent_terms=None):
+        self.req = np.zeros(0, dtype=abi.CREQ) if req is None else req
+        self.op_esc = np.zeros(0, dtype=abi.CESC_OP) if op_esc is None else op_esc
+        self.ent_terms = np.zeros(0, dtype=np.int64) if ent_terms is None else ent_terms
+        self.req_entries = int(((self.req["meta"] >> np.uint32(5)) & np.uint32(0x3F)).sum())
+
+    def nbytes(self):
+        return self.req.nbytes + self.op_esc.nbytes + self.ent_terms.nbytes
+
+    def as_c(self) -> abi.CReqsC:
+        c = abi.CReqsC()
+        c.n_req, c.n_op_esc = len(self.req), len(self.op_esc)
+        c.req = self.req.ctypes.data if len(self.req) else None
+        c.op_esc = self.op_esc.ctypes.data if len(self.op_esc) else None
+        c.ent_terms = self.ent_terms.ctypes.data if len(self.ent_terms) else None
+        c.ent_count, c.req_entries = len(self.ent_terms), self.req_entries
         return c
 
 
@@ -102,13 +125,60 @@ def inbox_in_block(block: np.ndarray, in_off, ci: CompactInbox) -> CompactInbox:
     return out
 
 
+def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray) -> tuple[CompactRequests, np.ndarray]:
+    """The request list of a dense inbox: every op other than a SUBMIT / TIMEOUT without a draw, in slot order.  Returns it
+    and the mask of the slots it carries (op_c leaves them NONE)."""
+    rows, n = ib.rows, ib.n
+    draw = ib.op_nr["y"]
+    listed = (ok != 0) & (((ok != abi.OP_SUBMIT) & (ok != abi.OP_TIMEOUT)) | (draw != 0))
+    at = np.flatnonzero(listed.reshape(-1))
+    if len(at) == 0:
+        return CompactRequests(), listed
+    meta = ib.op_meta.reshape(-1)[at]
+    kind = (meta & U64(0xFF)).astype(np.int64)
+    peer = ((meta >> U64(8)) & U64(0xFF)).astype(np.int64)
+    count = ((meta >> U64(16)) & U64(0xFFFF)).astype(np.int64)
+    ent = (meta >> U64(32)).astype(np.int64)
+    now, dr = ib.op_nr["x"].reshape(-1)[at], draw.reshape(-1)[at]
+    a, b = ib.op_ab["x"].reshape(-1)[at], ib.op_ab["y"].reshape(-1)[at]
+    cc = ib.op_cd["x"].reshape(-1)[at] if ib.op_cd is not None else np.zeros(len(at), np.int64)
+    d = ib.op_cd["y"].reshape(-1)[at] if ib.op_cd is not None else np.zeros(len(at), np.int64)
+    e = ib.op_e.reshape(-1)[at] if ib.op_e is not None else (b.astype(np.uint64) + U64(1)).astype(np.int64)
+    dt = now - base[at // n]
+    in_pool = ent + count <= ib.ent_count
+    wrap = lambda x: x.astype(np.uint64)                                        # int64 arithmetic modulo 2^64, as the engine's
+    dterm = wrap(a) - wrap(cc)
+    dcommit = (wrap(d) - wrap(b)).astype(np.int64)
+    fits = ((kind == abi.OP_AE_REQUEST) & (dr == 0) & (wrap(e) == wrap(b) + U64(1)) & (dterm < U64(1 << 32)) &
+            (dcommit >= -(1 << 31)) & (dcommit < (1 << 31)) & (dt >= 0) & (dt <= 0xFFFF) & (count <= 63) & (peer < 32) & in_pool)
+    for k in np.flatnonzero(fits & (count > 0)):                               # every entry carries the request's term
+        fits[k] = bool((ib.ent_terms[ent[k]:ent[k] + count[k]] == a[k]).all())
+    req = np.zeros(int(fits.sum()), dtype=abi.CREQ)
+    req["slot"] = at[fits]
+    req["meta"] = (peer[fits] | (count[fits] << 5) | (dt[fits] << 16)).astype(np.uint32)
+    req["term"], req["prev_index"] = a[fits], b[fits]
+    req["d_prev_term"], req["d_commit"] = dterm[fits].astype(np.uint32), dcommit[fits].astype(np.int32)
+    esc_k = np.flatnonzero(~fits)
+    op_esc = np.zeros(len(esc_k), dtype=abi.CESC_OP)
+    terms, pos = [], 0
+    for j, k in enumerate(esc_k):
+        off = 0xFFFFFFFF                                                        # out of the dense pool: out of this one too
+        if in_pool[k]:
+            off = pos
+            terms.append(ib.ent_terms[ent[k]:ent[k] + count[k]]); pos += int(count[k])
+        op_esc[j] = (at[k], off, int(meta[k]) & 0xFFFFFFFF, now[k], dr[k], a[k], b[k], cc[k], d[k], e[k])
+    return CompactRequests(req, op_esc, np.concatenate(terms).astype(np.int64) if terms else None), listed
+
+
 def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray | None, sent_inc: np.ndarray | None = None) -> CompactInbox:
-    """ib: dense host inbox of a NO_REQUESTS step (SUBMIT / TIMEOUT ops, any lane events).
+    """ib: dense host inbox (any group ops, any lane events).
     tags[r, i, f]: the tag the RPC this event answers was sent under (plan_c of the step that emitted it); None = no acks yet.
     sent_term[i] / sent_inc[i]: the term those RPCs carried and the incarnation of the role object that sent them (the group's
     current_term / incarnation columns of the step that planned them).  The incarnation is not on the wire — the engine keeps
     it with the echo pair under the tag — so a reply whose incarnation differs from sent_inc (a plan that was itself escaped)
-    travels in full."""
+    travels in full.
+    Inbound requests, and SUBMIT / TIMEOUT ops with an explicit election-timeout draw, go to the request list `.reqs`
+    (CompactRequests; None when the step has none: then it is a RAFTING_INBOX_NO_REQUESTS step)."""
     rows, n, F = ib.rows, ib.n, ib.F
     if ib.gids is not None:
         raise ValueError("the compact path is dense (no active list)")
@@ -116,8 +186,6 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     ek = (ib.ev_meta & U64(0xF)).astype(np.int64) if ib.ev_meta is not None else np.zeros((rows, n, F), np.int64)
     has_op = ib.op_meta is not None
     ok = (ib.op_meta & U64(0xFF)) if has_op else None
-    if has_op and (((ok != 0) & (ok != abi.OP_SUBMIT) & (ok != abi.OP_TIMEOUT)).any() or (ib.op_nr["y"] != 0).any()):
-        raise ValueError("the compact path carries SUBMIT / TIMEOUT ops without an explicit election-timeout draw only")
     # row base = the smallest time of the row
     big = np.iinfo(np.int64).max
     t_ev = np.where(ek != 0, ib.ev_tn["y"], big).reshape(rows, -1).min(axis=1) if ib.ev_meta is not None else np.full(rows, big)
@@ -125,14 +193,20 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     base = np.minimum(t_ev, t_op)
     base[base == big] = 0
     c.row_base[:] = base
+    c.reqs = None
     if has_op:
+        reqs, listed = _encode_requests(ib, ok, base)
+        if listed.any():
+            c.reqs = reqs
+            ok = np.where(listed, U64(0), ok)
         dt = np.where(ok != 0, ib.op_nr["x"] - base[:, None], 0)
         if (dt < 0).any() or (dt > 0xFFFF).any():
             raise ValueError("a group op lies more than 65.535 s after its row's base time: use the dense path for this step")
         unav = ib.op_ab["x"].astype(np.uint64) if ib.op_ab is not None else np.zeros((rows, n), np.uint64)
+        unav[listed] = 0
         if (unav > U64(0xFFFF)).any():
             raise ValueError("unavailable mask beyond 16 lanes")
-        count = (ib.op_meta >> U64(16)) & U64(0xFFFF)
+        count = np.where(listed, U64(0), (ib.op_meta >> U64(16)) & U64(0xFFFF))
         if (count > U64(0xFFF)).any():
             raise ValueError("more than 4095 commands in one SUBMIT: use the dense path for this step")
         c.op_c[:] = (ok | (count << U64(4)) | (dt.astype(np.uint64) << U64(16))).astype(np.uint32)
@@ -189,7 +263,10 @@ def decode_outbox(co: CompactOutbox, G: int | None = None) -> abi.Outbox:
     o.plan_lc["x"] = np.where(ae, prev + cnt, np.where(isn, ep["x"][None, :, None], 0))
     o.plan_lc["y"] = np.where(ae | isn, commit - dcommit, 0)
     o.plan_epoch[:] = np.where(kind != 0, ep["x"][None, :, None], 0)
-    o.rep_meta[:] = co.rep_c.astype(np.uint32) << np.uint32(8)
+    rc = co.rep_c.astype(np.uint32)
+    compact_rep = (rc >> np.uint32(7)) != 0                                   # a valid reply with the group's end-of-step term
+    o.rep_meta[:] = ((rc & np.uint32(0x3F)) << np.uint32(8)) | np.where(compact_rep, np.uint32(1) | (((rc >> np.uint32(6)) & np.uint32(1)) << np.uint32(1)), np.uint32(0))
+    o.rep_term[:] = np.where(compact_rep, co.current_term[None, :], 0)
     for name in ("commit_index", "current_term", "role_word", "incarnation", "err_word", "last_entry"):
         getattr(o, name)[:n] = getattr(co, name)
     for r in co.esc[:int(co.counts[0])]:

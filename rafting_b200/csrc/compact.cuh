@@ -15,6 +15,7 @@
 //
 // Included at the end of engine.cu (same translation unit: it uses rafting_engine, Slot, fail(), CU()).
 #pragma once
+#include <cub/device/device_scan.cuh>
 
 namespace rafting {
 
@@ -23,6 +24,7 @@ constexpr int CTAGS = 32;                        // in-flight slots per (group, 
 
 struct InboxW {                                  // writable view of the dense staging columns unpack_kernel fills
     uint64_t* op_meta; i64x2* op_nr; i64x2* op_ab; uint64_t* ev_meta; i64x2* ev_tn; i64x2* ev_el;
+    i64x2* op_cd; int64_t* op_e; int64_t* ent_terms;   // steps with a request list only, else null
 };
 struct CInD {                                    // device view of rafting_cinbox_t
     uint32_t rows, n_esc;
@@ -32,6 +34,7 @@ struct COutD {                                   // device view of rafting_coutb
     uint32_t* plan_c; uint8_t* rep_c;
     int64_t* commit_index; int64_t* current_term; uint32_t* role_word; uint32_t* incarnation; uint32_t* err_word;
     i64x2* last_entry; i64x2* epoch; rafting_cesc_out_t* esc; uint32_t esc_cap; uint32_t* counts;
+    bool compact_replies;                        // rep_c bits 6 / 7 (steps begun with a request list)
 };
 
 __global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW out, const i64x2* __restrict__ table, const uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits) {
@@ -59,16 +62,93 @@ __global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW o
         }
         bits[t] = b;
     }
-    if (f == 0 && in.op_c) {
+    if (f == 0 && (in.op_c || out.op_cd)) {
         for (uint32_t r = 0; r < in.rows; r++) {
             const size_t gi = (size_t)r * T.G + g;
-            const uint32_t c = in.op_c[gi];
+            const uint32_t c = in.op_c ? in.op_c[gi] : 0u;
             out.op_meta[gi] = (uint64_t)RAFTING_OP_MAKE(c & 0xfu, 0u, (c >> 4) & 0xfffu);
             i64x2 nr; nr.x = in.row_base[r] + (int64_t)(c >> 16); nr.y = 0;
             out.op_nr[gi] = nr;
             if (out.op_ab) { i64x2 ab; ab.x = in.op_unavail ? (int64_t)in.op_unavail[gi] : 0; ab.y = 0; out.op_ab[gi] = ab; }
+            if (out.op_cd) { const i64x2 z = {0, 0}; out.op_cd[gi] = z; out.op_e[gi] = 0; }
         }
     }
+}
+
+// ---- the request list (rafting_creqs_t): records and op escapes, after unpack_kernel has written the op_c words ----
+struct CReqD {                                   // device view of rafting_creqs_t
+    uint32_t n_req, n_esc, slots;                // slots = rows * G
+    const rafting_creq_t* req; const rafting_cesc_op_t* esc;
+    const int64_t* row_base; const uint32_t* op_c;
+    uint32_t ent_count, pool_end;                // records' terms start at ent_count; the step's pool ends at pool_end
+    uint64_t* counts; uint64_t* offs;            // [n_req] entry count of each record, its exclusive scan
+    uint32_t* order;                             // bit 0: req decreases somewhere, bit 1: esc does
+};
+constexpr uint32_t CREQ_META_ZERO = 0xf800u;     // bits 11..15 of a record's meta
+
+// Pass 1, one thread per list position: entry counts for the scan, and whether either list decreases anywhere.  A
+// decreasing list can hold the same slot twice at positions that are not adjacent; rather than search for them, every
+// op of both lists is then malformed, so that all writers of a slot write the same thing.
+__global__ void creq_prepare_kernel(CReqD q) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < q.n_req) {
+        q.counts[k] = RAFTING_CREQ_COUNT(q.req[k].meta);
+        if (k + 1 < q.n_req && q.req[k + 1].slot < q.req[k].slot) atomicOr(q.order, 1u);
+    }
+    if (k + 1 < q.n_esc && q.esc[k + 1].slot < q.esc[k].slot) atomicOr(q.order, 2u);
+}
+
+template <typename Rec> __device__ __forceinline__ bool list_holds(const Rec* v, uint32_t n, uint32_t slot) {
+    uint32_t lo = 0, hi = n;                     // binary search of a non-decreasing list
+    while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (v[m].slot < slot) lo = m + 1; else hi = m; }
+    return lo < n && v[lo].slot == slot;
+}
+
+__device__ __forceinline__ void put_op(const InboxW& o, size_t gi, uint64_t meta, int64_t now, int64_t draw, int64_t a, int64_t b,
+                                       int64_t c, int64_t d, int64_t e) {
+    o.op_meta[gi] = meta;
+    i64x2 v; v.x = now; v.y = draw; o.op_nr[gi] = v;
+    v.x = a; v.y = b; o.op_ab[gi] = v;
+    v.x = c; v.y = d; o.op_cd[gi] = v;
+    o.op_e[gi] = e;
+}
+
+// Pass 2, one thread per record (k < n_req) or op escape (k - n_req): the op in full at its slot.  Every writer of a slot
+// that is claimed twice detects it from read-only inputs and writes the same malformed op, so the result never depends on
+// the order of the writes.
+__global__ void unpack_requests_kernel(CReqD q, InboxW o, uint32_t G) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if ((uint64_t)k >= (uint64_t)q.n_req + q.n_esc) return;
+    const bool is_req = k < q.n_req;
+    const uint32_t j = is_req ? k : k - q.n_req;
+    const uint32_t slot = is_req ? q.req[j].slot : q.esc[j].slot;
+    if (slot >= q.slots) return;
+    const uint32_t r = slot / G;
+    bool bad = q.order[0] != 0 || (q.op_c && (q.op_c[slot] & 0xfu) != RAFTING_OP_NONE);
+    if (is_req) {
+        bad = bad || (j > 0 && q.req[j - 1].slot == slot) || (j + 1 < q.n_req && q.req[j + 1].slot == slot) ||
+              list_holds(q.esc, q.n_esc, slot) || (q.req[j].meta & CREQ_META_ZERO) != 0;
+    } else {
+        bad = bad || (j > 0 && q.esc[j - 1].slot == slot) || (j + 1 < q.n_esc && q.esc[j + 1].slot == slot) ||
+              list_holds(q.req, q.n_req, slot);
+    }
+    if (bad) { put_op(o, slot, RAFTING_COP_MALFORMED, q.row_base[r], 0, 0, 0, 0, 0, 0); return; }
+    if (!is_req) {
+        const rafting_cesc_op_t x = q.esc[j];
+        put_op(o, slot, (uint64_t)(uint32_t)x.op_meta | ((uint64_t)x.ent << 32), x.now_ms, x.draw, x.a, x.b, x.c, x.d, x.e);
+        return;
+    }
+    const rafting_creq_t x = q.req[j];
+    const uint32_t count = RAFTING_CREQ_COUNT(x.meta);
+    const uint64_t off = (uint64_t)q.ent_count + q.offs[j];
+    if (off + count <= q.pool_end)
+        for (uint32_t i = 0; i < count; i++) o.ent_terms[off + i] = x.term;
+    const uint32_t ent = off < 0xffffffffull ? (uint32_t)off : 0xffffffffu;   // past the pool: the step answers BAD_EVENT
+    const int64_t prev = x.prev_index;
+    put_op(o, slot, (uint64_t)RAFTING_OP_MAKE(RAFTING_OP_AE_REQUEST, RAFTING_CREQ_PEER(x.meta), count) | ((uint64_t)ent << 32),
+           q.row_base[r] + (int64_t)RAFTING_CREQ_DT(x.meta), 0, x.term, prev,
+           (int64_t)((uint64_t)x.term - (uint64_t)x.d_prev_term), (int64_t)((uint64_t)prev + (uint64_t)(int64_t)x.d_commit),
+           (int64_t)((uint64_t)prev + 1u));
 }
 // escape records: the event in full, after unpack_kernel has written the slot as empty
 __global__ void unpack_escapes_kernel(CInD in, InboxW out, uint32_t slots) {
@@ -139,8 +219,14 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
         for (uint32_t r = 0; r < rows; r++) {
             const size_t gi = (size_t)r * T.G + g;
             const uint32_t rm = in.rep_meta ? in.rep_meta[gi] : 0u;
-            out.rep_c[gi] = (uint8_t)RAFTING_REP_ERR(rm);
-            if (RAFTING_REP_VALID(rm)) { atomicAdd(out.counts + 2, 1u); put_escape(out, RAFTING_CESC_REPLY, (uint32_t)gi, rm, in.rep_term[gi], 0, 0, 0, 0); }
+            uint32_t rc = RAFTING_REP_ERR(rm);
+            if (RAFTING_REP_VALID(rm)) {
+                atomicAdd(out.counts + 2, 1u);
+                const int64_t rt = in.rep_term[gi];
+                if (out.compact_replies && rt == term_end) rc |= 0x80u | (RAFTING_REP_SUCCESS(rm) << 6);
+                else put_escape(out, RAFTING_CESC_REPLY, (uint32_t)gi, rm, rt, 0, 0, 0, 0);
+            }
+            out.rep_c[gi] = (uint8_t)rc;
             const uint64_t bm = in.ballot_meta ? in.ballot_meta[gi] : 0ull;
             if (bm != 0) { atomicAdd(out.counts + 1, 1u); const i64x2 bl = in.ballot_last[gi]; put_escape(out, RAFTING_CESC_BALLOT, (uint32_t)gi, bm, in.ballot_term[gi], bl.x, bl.y, 0, 0); }
         }
@@ -204,10 +290,37 @@ extern "C" int rafting_compact_layout(uint32_t rows, uint32_t G, uint32_t F, uin
     return RAFTING_OK;
 }
 
+// the request list's block: records, op escapes, then the entry pool (the device block extends the pool by the records' terms)
+struct CRLayout { size_t req, esc, ent, total; };
+static CRLayout compact_req_layout(size_t n_req, size_t n_esc, size_t ent_count) {
+    CRLayout L; size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; };
+    L.req = take(n_req * sizeof(rafting_creq_t)); L.esc = take(n_esc * sizeof(rafting_cesc_op_t)); L.ent = o; o += ent_count * 8;
+    L.total = o;
+    return L;
+}
+extern "C" int rafting_compact_req_layout(uint32_t n_req, uint32_t n_op_esc, uint32_t ent_count, uint64_t off[4]) {
+    if (!off) return fail(RAFTING_E_INVAL, "null argument");
+    const CRLayout L = compact_req_layout(n_req, n_op_esc, ent_count);
+    off[0] = L.req; off[1] = L.esc; off[2] = L.ent; off[3] = L.total;
+    return RAFTING_OK;
+}
+
 extern "C" int rafting_step_begin_compact(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_coutbox_t* out) {
+    return rafting_step_begin_compact_req(e, slot, in, nullptr, out);
+}
+
+extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
+                                              const rafting_coutbox_t* out) {
     using namespace rafting;
     if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
-    if (!in->row_base || (!in->op_c && !in->ev_c)) return fail(RAFTING_E_INVAL, "compact inbox needs row_base and at least one of op_c / ev_c");
+    const bool has_reqs = reqs && (reqs->n_req || reqs->n_op_esc);
+    if (!in->row_base || (!in->op_c && !in->ev_c && !has_reqs))
+        return fail(RAFTING_E_INVAL, "compact inbox needs row_base and at least one of op_c / ev_c / a request");
+    if (reqs && ((reqs->n_req && !reqs->req) || (reqs->n_op_esc && !reqs->op_esc) || (reqs->ent_count && !reqs->ent_terms)))
+        return fail(RAFTING_E_INVAL, "request list: a count without its array");
+    if (reqs && (uint64_t)reqs->ent_count + reqs->req_entries > e->cfg.entry_pool_cap)
+        return fail(RAFTING_E_CAPACITY, "ent_count + req_entries > entry_pool_cap");
     if (in->n_esc && !in->esc) return fail(RAFTING_E_INVAL, "n_esc without esc");
     if (!out->plan_c || !out->rep_c || !out->commit_index || !out->current_term || !out->role_word || !out->incarnation ||
         !out->err_word || !out->last_entry || !out->epoch || !out->counts || (out->esc_cap && !out->esc))
@@ -222,11 +335,22 @@ extern "C" int rafting_step_begin_compact(rafting_engine_t* e, uint32_t slot, co
     if (S.inflight) return fail(RAFTING_E_BUSY, "slot %u has a step in flight", slot);
     const size_t rows = in->rows, G = e->G, F = e->F;
     if (rows == 0 || rows > e->cfg.max_rows) return fail(RAFTING_E_CAPACITY, "rows %zu beyond max_rows %u", rows, e->cfg.max_rows);
-    const Layout LD = make_layout(rows, G, F, G, 0, 0);                        // dense staging the step kernel works on
+    const size_t n_req = has_reqs ? reqs->n_req : 0, n_oesc = has_reqs ? reqs->n_op_esc : 0;
+    if (has_reqs && (uint64_t)rows * G * F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
+    if (n_req > rows * G || n_oesc > rows * G || n_req > 0x7fffffffu)
+        return fail(RAFTING_E_INVAL, "a request list longer than rows * G cannot be strictly increasing");
+    const size_t ent_esc = has_reqs ? reqs->ent_count : 0, pool = has_reqs ? ent_esc + reqs->req_entries : 0;
+    const Layout LD = make_layout(rows, G, F, G, 0, 0);                        // dense staging the step kernel works on (the
+                                                                               // entry pool lives in the request block)
     const CLayout LC = compact_layout(rows, G, F, in->n_esc, out->esc_cap);
+    const CRLayout LR = compact_req_layout(n_req, n_oesc, ent_esc);
+    size_t scan_tmp = 0;
+    if (n_req) CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n_req));
+    const size_t w_counts = 256, w_offs = w_counts + ((n_req * 8 + 255) & ~(size_t)255), w_tmp = w_offs + ((n_req * 8 + 255) & ~(size_t)255);
     if ((rc = blk_reserve(S.din, LD.in_total, false)) || (rc = blk_reserve(S.dout, LD.out_total, false)) ||
         (rc = blk_reserve(S.cin, LC.in_total, false)) || (rc = blk_reserve(S.cout, LC.out_total, false)) ||
         (rc = blk_reserve(S.chout, 256, true))) return rc;
+    if (has_reqs && ((rc = blk_reserve(S.creq, LR.ent + pool * 8, false)) || (rc = blk_reserve(S.creqw, w_tmp + scan_tmp, false)))) return rc;
     // ---- H2D: the wire columns as they are ----
     CInD ci; ci.rows = (uint32_t)rows; ci.n_esc = in->n_esc;
     ci.row_base = (const int64_t*)(S.cin.p + LC.row_base); ci.op_c = nullptr; ci.op_unavail = nullptr; ci.ev_c = nullptr;
@@ -250,13 +374,28 @@ extern "C" int rafting_step_begin_compact(rafting_engine_t* e, uint32_t slot, co
             if (in->n_esc) CU(cudaMemcpyAsync(S.cin.p + LC.esc, in->esc, (size_t)in->n_esc * sizeof(rafting_cesc_in_t), cudaMemcpyHostToDevice, H->s_h2d));
         }
     }
+    if (has_reqs) {                                                            // the request list: one copy when carved as laid out
+        const uint8_t* hb = n_req ? (const uint8_t*)reqs->req - LR.req : (const uint8_t*)reqs->op_esc - LR.esc;
+        const bool one_block = (!n_req || (const uint8_t*)reqs->req == hb + LR.req) && (!n_oesc || (const uint8_t*)reqs->op_esc == hb + LR.esc) &&
+                               (!ent_esc || (const uint8_t*)reqs->ent_terms == hb + LR.ent);
+        if (one_block) CU(cudaMemcpyAsync(S.creq.p, hb, LR.total, cudaMemcpyHostToDevice, H->s_h2d));
+        else {
+            if (n_req) CU(cudaMemcpyAsync(S.creq.p + LR.req, reqs->req, n_req * sizeof(rafting_creq_t), cudaMemcpyHostToDevice, H->s_h2d));
+            if (n_oesc) CU(cudaMemcpyAsync(S.creq.p + LR.esc, reqs->op_esc, n_oesc * sizeof(rafting_cesc_op_t), cudaMemcpyHostToDevice, H->s_h2d));
+            if (ent_esc) CU(cudaMemcpyAsync(S.creq.p + LR.ent, reqs->ent_terms, ent_esc * 8, cudaMemcpyHostToDevice, H->s_h2d));
+        }
+    }
     CU(cudaEventRecord(S.ev_h2d, H->s_h2d));
     // ---- unpack -> step -> pack on the engine's stream ----
     InboxD di; memset(&di, 0, sizeof(di));
-    di.rows = (uint32_t)rows; di.n = (uint32_t)G; di.flags = RAFTING_INBOX_NO_REQUESTS;
-    if (in->op_c) {
+    di.rows = (uint32_t)rows; di.n = (uint32_t)G; di.flags = has_reqs ? 0u : RAFTING_INBOX_NO_REQUESTS;
+    if (in->op_c || has_reqs) {
         di.op_meta = (const uint64_t*)(S.din.p + LD.in_off[2]); di.op_nr = (const i64x2*)(S.din.p + LD.in_off[3]);
-        if (in->op_unavail) di.op_ab = (const i64x2*)(S.din.p + LD.in_off[4]);   // else nobody is unavailable
+        if (in->op_unavail || has_reqs) di.op_ab = (const i64x2*)(S.din.p + LD.in_off[4]);   // else nobody is unavailable
+    }
+    if (has_reqs) {
+        di.op_cd = (const i64x2*)(S.din.p + LD.in_off[5]); di.op_e = (const int64_t*)(S.din.p + LD.in_off[6]);
+        di.ent_terms = (const int64_t*)(S.creq.p + LR.ent); di.ent_count = (uint32_t)pool;
     }
     if (in->ev_c || in->n_esc) {
         di.ev_meta = (const uint64_t*)(S.din.p + LD.in_off[8]); di.ev_tn = (const i64x2*)(S.din.p + LD.in_off[9]); di.ev_el = (const i64x2*)(S.din.p + LD.in_off[10]);
@@ -271,13 +410,13 @@ extern "C" int rafting_step_begin_compact(rafting_engine_t* e, uint32_t slot, co
     dov.incarnation = (uint32_t*)(S.dout.p + LD.out_off[12]); dov.err_word = (uint32_t*)(S.dout.p + LD.out_off[13]);
     dov.last_entry = (i64x2*)(S.dout.p + LD.out_off[14]);
     dov.flags = (uint32_t*)(S.dout.p + LD.flags_off);
-    if (!in->op_c) { dov.rep_meta = nullptr; dov.rep_term = nullptr; dov.plan_meta = nullptr; dov.plan_pp = nullptr; dov.plan_lc = nullptr; dov.plan_epoch = nullptr; }
+    if (!in->op_c && !has_reqs) { dov.rep_meta = nullptr; dov.rep_term = nullptr; dov.plan_meta = nullptr; dov.plan_pp = nullptr; dov.plan_lc = nullptr; dov.plan_epoch = nullptr; }
     COutD co;
     co.plan_c = (uint32_t*)(S.cout.p + LC.plan_c); co.rep_c = (uint8_t*)(S.cout.p + LC.rep_c);
     co.commit_index = (int64_t*)(S.cout.p + LC.commit); co.current_term = (int64_t*)(S.cout.p + LC.term); co.role_word = (uint32_t*)(S.cout.p + LC.role);
     co.incarnation = (uint32_t*)(S.cout.p + LC.inc); co.err_word = (uint32_t*)(S.cout.p + LC.err); co.last_entry = (i64x2*)(S.cout.p + LC.last);
     co.epoch = (i64x2*)(S.cout.p + LC.epoch); co.counts = (uint32_t*)(S.cout.p + LC.counts);
-    co.esc = (rafting_cesc_out_t*)(S.cout.p + LC.esc_out); co.esc_cap = out->esc_cap;
+    co.esc = (rafting_cesc_out_t*)(S.cout.p + LC.esc_out); co.esc_cap = out->esc_cap; co.compact_replies = reqs != nullptr;
     const uint32_t GF = (uint32_t)(G * F), blocks = (GF + 255u) / 256u;
     CU(cudaStreamWaitEvent(e->stream, S.ev_h2d, 0));
     CU(cudaMemsetAsync(dov.flags, 0, 16, e->stream));
@@ -285,9 +424,23 @@ extern "C" int rafting_step_begin_compact(rafting_engine_t* e, uint32_t slot, co
     InboxW dw;                                                                 // unpack writes what the step kernel reads
     dw.op_meta = (uint64_t*)di.op_meta; dw.op_nr = (i64x2*)di.op_nr; dw.op_ab = (i64x2*)di.op_ab;
     dw.ev_meta = (uint64_t*)di.ev_meta; dw.ev_tn = (i64x2*)di.ev_tn; dw.ev_el = (i64x2*)di.ev_el;
+    dw.op_cd = (i64x2*)di.op_cd; dw.op_e = (int64_t*)di.op_e; dw.ent_terms = (int64_t*)di.ent_terms;
     unpack_kernel<<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits);
     if (in->ev_c == nullptr && in->n_esc) CU(cudaMemsetAsync((void*)di.ev_meta, 0, rows * G * F * 8, e->stream));
     if (in->n_esc) unpack_escapes_kernel<<<(in->n_esc + 255u) / 256u, 256, 0, e->stream>>>(ci, dw, (uint32_t)(rows * G * F));
+    if (has_reqs) {
+        CReqD q;
+        q.n_req = (uint32_t)n_req; q.n_esc = (uint32_t)n_oesc; q.slots = (uint32_t)(rows * G);
+        q.req = (const rafting_creq_t*)(S.creq.p + LR.req); q.esc = (const rafting_cesc_op_t*)(S.creq.p + LR.esc);
+        q.row_base = ci.row_base; q.op_c = ci.op_c;
+        q.ent_count = (uint32_t)ent_esc; q.pool_end = (uint32_t)pool;
+        q.order = (uint32_t*)S.creqw.p; q.counts = (uint64_t*)(S.creqw.p + w_counts); q.offs = (uint64_t*)(S.creqw.p + w_offs);
+        const uint32_t most = (uint32_t)(n_req > n_oesc ? n_req : n_oesc);
+        CU(cudaMemsetAsync(q.order, 0, 4, e->stream));
+        creq_prepare_kernel<<<(most + 255u) / 256u, 256, 0, e->stream>>>(q);
+        if (n_req) { size_t tb = scan_tmp; CU(cub::DeviceScan::ExclusiveSum(S.creqw.p + w_tmp, tb, q.counts, q.offs, (int)n_req, e->stream)); }
+        unpack_requests_kernel<<<(uint32_t)((n_req + n_oesc + 255u) / 256u), 256, 0, e->stream>>>(q, dw, (uint32_t)G);
+    }
     CU(cudaGetLastError());
     rc = launch_step(e, di, dov, e->stream);
     if (rc) { cudaStreamSynchronize(H->s_h2d); return rc; }

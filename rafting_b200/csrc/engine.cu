@@ -464,7 +464,8 @@ static int blk_reserve(Blk& b, size_t bytes, bool pinned) {
 struct Slot {
     Blk din, dout;                            // device staging (both paths)
     Blk cin, cout, chin, chout;               // compact path: device wire blocks + pinned landing block of the small items
-    bool compact_step = false;                // the step in flight came through rafting_step_begin_compact
+    Blk creq, creqw;                          // compact path: request list + entry pool, and its scan scratch
+    bool compact_step = false;                // the step in flight came through rafting_step_begin_compact[_req]
     rafting_coutbox_t c_host; size_t c_esc_off = 0; uint32_t* c_counts_pinned = nullptr; void* c_esc_dev = nullptr;
     Blk hin, hout;                            // pinned host staging (leases only), same layout as din / dout
     uint32_t* h_flags = nullptr;              // pinned landing place of the flag words on the caller-owned path
@@ -518,6 +519,8 @@ static void hostpath_free(rafting_engine* e) {
         if (s.cout.p) cudaFree(s.cout.p);
         if (s.chin.p) cudaFreeHost(s.chin.p);
         if (s.chout.p) cudaFreeHost(s.chout.p);
+        if (s.creq.p) cudaFree(s.creq.p);
+        if (s.creqw.p) cudaFree(s.creqw.p);
         if (s.ev_h2d) cudaEventDestroy(s.ev_h2d);
         if (s.ev_kernel) cudaEventDestroy(s.ev_kernel);
         if (s.ev_done) cudaEventDestroy(s.ev_done);

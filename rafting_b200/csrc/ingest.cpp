@@ -3,6 +3,7 @@
 
 #include <string.h>
 
+#include <algorithm>
 #include <deque>
 #include <vector>
 
@@ -403,6 +404,103 @@ extern "C" int rafting_outbox_to_replies(const rafting_outbox_t* ob, uint32_t n_
         r.flags = (uint8_t)(RAFTING_OUT_OK | (RAFTING_REP_SUCCESS(m) << 2));
         r.incarnation = q.incarnation;
         r.term = ob->rep_term[gi];
+        r.epoch_at_send = q.epoch; r.last_at_send = q.last;
+        out[k++] = r;
+    }
+    *n_out = k;
+    return RAFTING_OK;
+}
+
+// ---- the same two ends of the loop for the compact host path (rafting_creqs_t in, rep_c out) ----
+namespace {
+template <typename Rec> uint32_t lower_slot(const Rec* v, uint32_t n, uint32_t slot) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t m = (lo + hi) / 2; if (v[m].slot < slot) lo = m + 1; else hi = m; }
+    return lo;
+}
+// inserts x at its place in a strictly increasing list (appending when the pump places in slot order)
+template <typename Rec> void insert_at(Rec* v, uint32_t* n, uint32_t at, const Rec& x) {
+    if (at < *n) memmove(v + at + 1, v + at, (size_t)(*n - at) * sizeof(Rec));
+    v[at] = x; (*n)++;
+}
+}  // namespace
+
+extern "C" int rafting_request_to_creq(const rafting_req_rec_t* r, const int64_t* entry_terms, uint32_t row, int64_t now_ms,
+                                       int host_result, const rafting_cinbox_t* in, uint32_t n_groups, rafting_creqs_t* q,
+                                       uint32_t req_cap, uint32_t esc_cap, uint32_t ent_cap) {
+    if (!r || !in || !in->row_base || !q || (q->n_req && !q->req) || (q->n_op_esc && !q->op_esc)) return RAFTING_E_INVAL;
+    if (r->gid >= n_groups || row >= in->rows) return RAFTING_E_INVAL;
+    if (r->kind != RAFTING_OP_AE_REQUEST && r->kind != RAFTING_OP_PREVOTE_REQ && r->kind != RAFTING_OP_VOTE_REQ &&
+        r->kind != RAFTING_OP_IS_REQUEST) return RAFTING_E_INVAL;
+    const uint32_t slot = row * n_groups + r->gid;
+    rafting_creq_t* req = const_cast<rafting_creq_t*>(q->req);
+    rafting_cesc_op_t* esc = const_cast<rafting_cesc_op_t*>(q->op_esc);
+    const uint32_t at_req = lower_slot(req, q->n_req, slot), at_esc = lower_slot(esc, q->n_op_esc, slot);
+    if ((in->op_c && (in->op_c[slot] & 0xfu) != RAFTING_OP_NONE) || (at_req < q->n_req && req[at_req].slot == slot) ||
+        (at_esc < q->n_op_esc && esc[at_esc].slot == slot)) return RAFTING_E_INVAL;            // one op per (row, group)
+    const bool ae = r->kind == RAFTING_OP_AE_REQUEST;
+    const uint32_t count = ae ? r->count : 0;
+    if (count > 0xFFFFu || (count && !entry_terms)) return RAFTING_E_INVAL;
+    const int64_t dt = now_ms - in->row_base[row];
+    const uint64_t dterm = (uint64_t)r->term - (uint64_t)r->b;
+    const int64_t dcommit = (int64_t)((uint64_t)r->commit - (uint64_t)r->a);
+    bool fits = ae && count <= 63 && r->src_slot < 32 && dt >= 0 && dt <= 0xFFFF && dterm < (1ull << 32) &&
+                dcommit >= INT32_MIN && dcommit <= INT32_MAX;
+    for (uint32_t i = 0; fits && i < count; i++) fits = entry_terms[i] == r->term;
+    if (fits) {
+        if (q->n_req >= req_cap) return RAFTING_E_INVAL;
+        rafting_creq_t x;
+        x.slot = slot; x.meta = RAFTING_CREQ_MAKE(r->src_slot, count, (uint32_t)dt); x.term = r->term; x.prev_index = r->a;
+        x.d_prev_term = (uint32_t)dterm; x.d_commit = (int32_t)dcommit;
+        insert_at(req, &q->n_req, at_req, x);
+        q->req_entries += count;
+        return RAFTING_OK;
+    }
+    // in full, as rafting_request_to_inbox writes the dense op slot
+    if (q->n_op_esc >= esc_cap || (count && (!q->ent_terms || (uint64_t)q->ent_count + count > ent_cap))) return RAFTING_E_INVAL;
+    rafting_cesc_op_t x;
+    memset(&x, 0, sizeof(x));
+    x.slot = slot; x.ent = q->ent_count; x.op_meta = RAFTING_OP_MAKE(r->kind, r->src_slot, count);
+    x.now_ms = now_ms; x.a = r->term; x.b = r->a; x.c = r->b;
+    if (ae) { x.d = r->commit; x.e = r->a + 1; }
+    else if (r->kind == RAFTING_OP_IS_REQUEST) x.d = host_result ? 1 : 0;
+    if (count) { memcpy(const_cast<int64_t*>(q->ent_terms) + q->ent_count, entry_terms, (size_t)count * 8); q->ent_count += count; }
+    insert_at(esc, &q->n_op_esc, at_esc, x);
+    return RAFTING_OK;
+}
+
+extern "C" int rafting_coutbox_to_replies(const rafting_coutbox_t* co, uint32_t n_groups, uint32_t local_slot,
+                                          const rafting_req_rec_t* placed, const uint8_t* placed_row, uint32_t n,
+                                          rafting_batch_rec_t* out, uint32_t* n_out) {
+    if (!co || !co->rep_c || !co->current_term || !co->counts || (!placed && n) || (!placed_row && n) || !out || !n_out) return RAFTING_E_INVAL;
+    if (co->counts[0] > co->esc_cap) return RAFTING_E_CAPACITY;               // the escape list overflowed: use the dense outbox
+    if (co->counts[0] && !co->esc) return RAFTING_E_INVAL;
+    std::vector<std::pair<uint32_t, uint32_t>> esc;                          // (slot, index) of the reply escapes, sorted
+    for (uint32_t k = 0; k < co->counts[0]; k++)
+        if (co->esc[k].kind == RAFTING_CESC_REPLY) esc.push_back({co->esc[k].slot, k});
+    std::sort(esc.begin(), esc.end());
+    uint32_t k = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const rafting_req_rec_t& q = placed[i];
+        if (q.gid >= n_groups || q.src_slot == local_slot) return RAFTING_E_INVAL;
+        const uint32_t gi = (uint32_t)placed_row[i] * n_groups + q.gid;
+        const uint8_t rc = co->rep_c[gi];
+        int64_t term; uint32_t success;
+        if (rc & 0x80u) { term = co->current_term[q.gid]; success = (rc >> 6) & 1u; }
+        else {
+            const auto it = std::lower_bound(esc.begin(), esc.end(), std::make_pair(gi, 0u));
+            if (it == esc.end() || it->first != gi) continue;                 // no valid reply: the handler threw
+            const rafting_cesc_out_t& e = co->esc[it->second];
+            term = e.a; success = RAFTING_REP_SUCCESS(e.meta);
+        }
+        rafting_batch_rec_t r{};
+        r.gid = q.gid;
+        r.kind = (uint8_t)(q.kind == RAFTING_OP_AE_REQUEST ? RAFTING_EV_AE_ACK : q.kind == RAFTING_OP_IS_REQUEST ? RAFTING_EV_IS_ACK
+                         : q.kind == RAFTING_OP_PREVOTE_REQ ? RAFTING_EV_PV_REPLY : RAFTING_EV_RV_REPLY);
+        r.lane = (uint8_t)(local_slot < q.src_slot ? local_slot : local_slot - 1);
+        r.flags = (uint8_t)(RAFTING_OUT_OK | (success << 2));
+        r.incarnation = q.incarnation;
+        r.term = term;
         r.epoch_at_send = q.epoch; r.last_at_send = q.last;
         out[k++] = r;
     }

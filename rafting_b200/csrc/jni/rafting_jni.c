@@ -111,6 +111,11 @@ JNIEXPORT void JNICALL FN(stepWaitSlot)(JNIEnv* env, jclass k, jlong h, jint slo
 JNIEXPORT void JNICALL FN(stepBeginCompact)(JNIEnv* env, jclass k, jlong h, jint slot, jobject cin, jobject cout) {
     CHECK(rafting_step_begin_compact(ENG(h), (uint32_t)slot, (const rafting_cinbox_t*)BUF(cin), (const rafting_coutbox_t*)BUF(cout)));
 }
+/* ... with the inbound requests of the step (a rafting_creqs_t struct in a direct buffer; null = none, as stepBeginCompact) */
+JNIEXPORT void JNICALL FN(stepBeginCompactReq)(JNIEnv* env, jclass k, jlong h, jint slot, jobject cin, jobject creqs, jobject cout) {
+    CHECK(rafting_step_begin_compact_req(ENG(h), (uint32_t)slot, (const rafting_cinbox_t*)BUF(cin), (const rafting_creqs_t*)BUF(creqs),
+                                         (const rafting_coutbox_t*)BUF(cout)));
+}
 JNIEXPORT void JNICALL FN(stepWaitCompact)(JNIEnv* env, jclass k, jlong h, jint slot) { CHECK(rafting_step_wait_compact(ENG(h), (uint32_t)slot)); }
 JNIEXPORT void JNICALL FN(stepFetchDense)(JNIEnv* env, jclass k, jlong h, jint slot, jobject outStruct) {
     CHECK(rafting_step_fetch_dense(ENG(h), (uint32_t)slot, (const rafting_outbox_t*)BUF(outStruct)));
@@ -259,6 +264,22 @@ JNIEXPORT jint JNICALL FN(outboxToReplies)(JNIEnv* env, jclass k, jobject outStr
     CHECK(rafting_outbox_to_replies((const rafting_outbox_t*)BUF(outStruct), (uint32_t)nGroups, (uint32_t)localSlot,
                                     (const rafting_req_rec_t*)BUF(placed), (const uint8_t*)BUF(placedRow), (uint32_t)n,
                                     (rafting_batch_rec_t*)BUF(repliesOut), &got));
+    return (jint)got;
+}
+/* the same two ends for the compact host path: a record into the step's request list (its counts grow in the struct), and
+   the replies of a waited-for compact outbox */
+JNIEXPORT void JNICALL FN(requestToCreq)(JNIEnv* env, jclass k, jobject rec, jobject entryTerms, jint row, jlong nowMs, jboolean hostResult,
+                                         jobject cinStruct, jint nGroups, jobject creqsStruct, jint reqCap, jint escCap, jint entCap) {
+    CHECK(rafting_request_to_creq((const rafting_req_rec_t*)BUF(rec), (const int64_t*)BUF(entryTerms), (uint32_t)row, nowMs, hostResult ? 1 : 0,
+                                  (const rafting_cinbox_t*)BUF(cinStruct), (uint32_t)nGroups, (rafting_creqs_t*)BUF(creqsStruct),
+                                  (uint32_t)reqCap, (uint32_t)escCap, (uint32_t)entCap));
+}
+JNIEXPORT jint JNICALL FN(coutboxToReplies)(JNIEnv* env, jclass k, jobject coutStruct, jint nGroups, jint localSlot, jobject placed,
+                                            jobject placedRow, jint n, jobject repliesOut) {
+    uint32_t got = 0;
+    CHECK(rafting_coutbox_to_replies((const rafting_coutbox_t*)BUF(coutStruct), (uint32_t)nGroups, (uint32_t)localSlot,
+                                     (const rafting_req_rec_t*)BUF(placed), (const uint8_t*)BUF(placedRow), (uint32_t)n,
+                                     (rafting_batch_rec_t*)BUF(repliesOut), &got));
     return (jint)got;
 }
 /* commit records of a step -> (gid, first, last) ranges for RaftMachine.apply; `applied` is the pump's long[G] in a direct buffer */

@@ -38,7 +38,7 @@ EXPORTS = [
     "rafting_comm_init", "rafting_comm_init_all", "rafting_comm_unique_id", "rafting_allgather_commit", "rafting_allgather_commit_from",
     "rafting_allgather_commit_all", "rafting_allgather_last", "rafting_restore_async", "rafting_state_save", "rafting_state_load", "rafting_step_device_seq", "rafting_engine_stream",
     "rafting_engine_counters", "rafting_abi_sizes", "rafting_checkpoint", "rafting_restore",
-    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
+    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
     "rafting_log_config", "rafting_log_append", "rafting_log_read", "rafting_log_gather", "rafting_log_trim", "rafting_log_stats",
     "rafting_log_store_open", "rafting_log_sync", "rafting_log_mark", "rafting_log_recovered", "rafting_log_export_kv", "rafting_log_store_stats",
 ]
@@ -113,6 +113,9 @@ def lib():
         L.rafting_step_begin_host.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.InboxC), C.POINTER(abi.OutboxC)]
         L.rafting_step_wait_slot.argtypes = [C.c_void_p, C.c_uint32]
         L.rafting_step_begin_compact.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.CInboxC), C.POINTER(abi.COutboxC)]
+        L.rafting_step_begin_compact_req.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.CInboxC), C.POINTER(abi.CReqsC),
+                                                     C.POINTER(abi.COutboxC)]
+        L.rafting_compact_req_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 4)]
         L.rafting_step_wait_compact.argtypes = [C.c_void_p, C.c_uint32]
         L.rafting_compact_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 6),
                                              C.POINTER(C.c_uint64 * 12)]
@@ -226,9 +229,24 @@ class Engine:
         _check(lib().rafting_compact_layout(rows, G, F, n_esc_in, esc_cap, C.byref(a), C.byref(b)), "rafting_compact_layout")
         return list(a), list(b)
 
-    def step_compact(self, cin, cout, slot: int = 0):
-        """Synchronous compact step: cin / cout are rafting_b200.compact.CompactInbox / CompactOutbox."""
-        self.step_begin_compact(slot, cin.as_c(), cout.as_c())
+    def step_begin_compact_req(self, slot: int, cin_c: abi.CInboxC, reqs_c: abi.CReqsC | None, cout_c: abi.COutboxC):
+        _check(lib().rafting_step_begin_compact_req(self._h, slot, C.byref(cin_c), None if reqs_c is None else C.byref(reqs_c),
+                                                    C.byref(cout_c)), "rafting_step_begin_compact_req")
+
+    @staticmethod
+    def compact_req_layout(n_req: int, n_op_esc: int, ent_count: int):
+        """-> byte offsets of req, op_esc, ent_terms and the block size (rafting_compact_req_layout)"""
+        a = (C.c_uint64 * 4)()
+        _check(lib().rafting_compact_req_layout(n_req, n_op_esc, ent_count, C.byref(a)), "rafting_compact_req_layout")
+        return list(a)
+
+    def step_compact(self, cin, cout, slot: int = 0, reqs=None):
+        """Synchronous compact step: cin / cout are rafting_b200.compact.CompactInbox / CompactOutbox, reqs a
+        rafting_b200.compact.CompactRequests (None: rafting_step_begin_compact)."""
+        if reqs is None:
+            self.step_begin_compact(slot, cin.as_c(), cout.as_c())
+        else:
+            self.step_begin_compact_req(slot, cin.as_c(), reqs.as_c(), cout.as_c())
         self.step_wait_compact(slot)
         return cout
 

@@ -55,6 +55,10 @@ def lib():
                                                C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]
         L.rafting_outbox_to_replies.argtypes = [C.POINTER(abi.OutboxC), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
                                                 C.c_void_p, C.POINTER(C.c_uint32)]
+        L.rafting_request_to_creq.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int64, C.c_int, C.POINTER(abi.CInboxC),
+                                              C.c_uint32, C.POINTER(abi.CReqsC), C.c_uint32, C.c_uint32, C.c_uint32]
+        L.rafting_coutbox_to_replies.argtypes = [C.POINTER(abi.COutboxC), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
+                                                 C.c_void_p, C.POINTER(C.c_uint32)]
         L.rafting_outbox_apply_ranges.argtypes = [C.POINTER(abi.OutboxC), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
                                                   C.c_uint32, C.POINTER(C.c_uint32)]
         L.rafting_pending_create.argtypes = [C.c_uint32, C.POINTER(C.c_void_p)]
@@ -230,6 +234,46 @@ def outbox_to_replies(outbox: abi.Outbox, n_groups: int, local_slot: int, placed
                                          out.ctypes.data, C.byref(n))
     if rc:
         raise ValueError(f"rafting_outbox_to_replies: rc={rc}")
+    return out[:n.value]
+
+
+class CReqPlacer:
+    """The request list of one compact step, filled by rafting_request_to_creq (the compact analogue of request_to_inbox)."""
+
+    def __init__(self, req_cap: int, esc_cap: int, ent_cap: int):
+        self.req = np.zeros(max(1, req_cap), dtype=abi.CREQ)
+        self.op_esc = np.zeros(max(1, esc_cap), dtype=abi.CESC_OP)
+        self.ent_terms = np.zeros(max(1, ent_cap), dtype=np.int64)
+        self.caps = (req_cap, esc_cap, ent_cap)
+        self.c = abi.CReqsC()
+        self.c.req, self.c.op_esc, self.c.ent_terms = self.req.ctypes.data, self.op_esc.ctypes.data, self.ent_terms.ctypes.data
+
+    def put(self, rec, entry_terms, row: int, now_ms: int, host_result: bool, cin, n_groups: int) -> int:
+        """One request record -> a record or an op escape at (row, rec.gid) of the compact step `cin`; returns the status code."""
+        r = np.array([rec], dtype=REQ_REC)
+        terms = np.ascontiguousarray(entry_terms, dtype=np.int64)
+        ic = cin.as_c()
+        return lib().rafting_request_to_creq(r.ctypes.data, terms.ctypes.data if len(terms) else None, row, now_ms, 1 if host_result else 0,
+                                             C.byref(ic), n_groups, C.byref(self.c), *self.caps)
+
+    def requests(self):
+        """-> rafting_b200.compact.CompactRequests (copies of the lists placed so far)"""
+        from .compact import CompactRequests
+        c = self.c
+        return CompactRequests(self.req[:c.n_req].copy(), self.op_esc[:c.n_op_esc].copy(), self.ent_terms[:c.ent_count].copy())
+
+
+def coutbox_to_replies(cout, n_groups: int, local_slot: int, placed: np.ndarray, placed_row) -> np.ndarray:
+    """outbox_to_replies over a compact outbox (rafting_b200.compact.CompactOutbox): replies from rep_c and the escape list."""
+    placed = np.ascontiguousarray(placed, dtype=REQ_REC)
+    rows = np.ascontiguousarray(placed_row, dtype=np.uint8)
+    out = np.zeros(max(1, len(placed)), dtype=BATCH_REC)
+    n = C.c_uint32()
+    oc = cout.as_c()
+    rc = lib().rafting_coutbox_to_replies(C.byref(oc), n_groups, local_slot, placed.ctypes.data, rows.ctypes.data, len(placed),
+                                          out.ctypes.data, C.byref(n))
+    if rc:
+        raise ValueError(f"rafting_coutbox_to_replies: rc={rc}")
     return out[:n.value]
 
 

@@ -29,6 +29,7 @@ final class NativeEngine {
     static native void stepBeginHost(long h, int slot, ByteBuffer inboxStruct, ByteBuffer outboxStruct);   // rafting_step_begin_host: Netty's pinned receive pool
     static native void stepWaitSlot(long h, int slot);                                           // rafting_step_wait_slot
     static native void stepBeginCompact(long h, int slot, ByteBuffer cinbox, ByteBuffer coutbox); // rafting_step_begin_compact (§7)
+    static native void stepBeginCompactReq(long h, int slot, ByteBuffer cinbox, ByteBuffer creqs, ByteBuffer coutbox);   // rafting_step_begin_compact_req: with inbound requests
     static native void stepWaitCompact(long h, int slot);                                        // rafting_step_wait_compact
     static native void stepFetchDense(long h, int slot, ByteBuffer outboxStruct);                // rafting_step_fetch_dense (escape overflow)
     static native void checkpoint(long h);                                                       // rafting_checkpoint
@@ -78,4 +79,7 @@ final class NativeEngine {
     static native int  outboxToRequests(long d, ByteBuffer outStruct, int rows, ByteBuffer reqRecsOut, int cap);   // plans + vote broadcasts -> 64 B request records
     static native int  requestToInbox(ByteBuffer rec, ByteBuffer entryTerms, int row, long nowMs, boolean hostResult, ByteBuffer inStruct, int nGroups, int entCap, int entCount);
     static native int  outboxToReplies(ByteBuffer outStruct, int nGroups, int localSlot, ByteBuffer placed, ByteBuffer placedRow, int n, ByteBuffer replyRecsOut);
+    static native void requestToCreq(ByteBuffer rec, ByteBuffer entryTerms, int row, long nowMs, boolean hostResult, ByteBuffer cinStruct, int nGroups,
+                                     ByteBuffer creqsStruct, int reqCap, int escCap, int entCap);   // a request record -> the compact step's request list
+    static native int  coutboxToReplies(ByteBuffer coutStruct, int nGroups, int localSlot, ByteBuffer placed, ByteBuffer placedRow, int n, ByteBuffer replyRecsOut);
 }
