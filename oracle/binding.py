@@ -100,10 +100,15 @@ class Oracle:
     def close_group(self, gid: int):
         lib().orc_group_close(self._h, gid)
 
-    def step(self, inbox: abi.Inbox, threads: int = 1) -> abi.Outbox:
+    def step(self, inbox: abi.Inbox, threads: int = 1, out: abi.Outbox | None = None) -> abi.Outbox:
+        """out: a caller-owned outbox to step into (cells the step does not write keep their bytes); None: a fresh
+        zeroed one."""
         n = inbox.n
         compact = inbox.gids is not None and (inbox.flags & abi.INBOX_COMPACT_GROUPS)
-        out = abi.Outbox(inbox.rows, n, self.F, n if compact else self.G)
+        if out is None:
+            out = abi.Outbox(inbox.rows, n, self.F, n if compact else self.G)
+        elif (out.rows, out.n, out.F, out.G) != (inbox.rows, n, self.F, n if compact else self.G):
+            raise ValueError("outbox shape does not match the inbox")
         ic, oc = inbox.as_c(), out.as_c()
         rc = lib().orc_step(self._h, C.byref(ic), C.byref(oc), threads)
         if rc:

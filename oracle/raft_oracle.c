@@ -949,6 +949,8 @@ static void step_row(orc_engine_t* e, const rafting_inbox_t* in, const rafting_o
         }
         int peer = (int)RAFTING_OP_PEER(meta); uint32_t count = RAFTING_OP_COUNT(meta);
         if (!g->alive) err = RAFTING_ERR_CLOSED_GROUP;
+        /* the caller promised no inbound requests: one found anyway is refused (rafting_b200.h, RAFTING_INBOX_NO_REQUESTS) */
+        else if (kind > RAFTING_OP_TIMEOUT && (in->flags & RAFTING_INBOX_NO_REQUESTS)) err = RAFTING_ERR_BAD_EVENT;
         else switch (kind) {
         case RAFTING_OP_SUBMIT:  err = op_submit(&c, count, (uint64_t)a); break;
         case RAFTING_OP_TIMEOUT: err = op_timeout(&c, (uint64_t)a); break;

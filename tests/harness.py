@@ -3,6 +3,7 @@ through the identical batch interface and compares outboxes and exported state b
 from __future__ import annotations
 
 import ctypes as C
+from dataclasses import dataclass, field
 
 import numpy as np
 
@@ -82,14 +83,35 @@ def run_leader_workload(suts, w: workload.WlCfg, steps: int, compare=True, first
 # random fuzz over every op / event kind, steered by the reference SUT's exported state
 # ---------------------------------------------------------------------------------------------
 class Fuzzer:
-    def __init__(self, cfg: abi.Cfg, ref, seed=1, rows=3, n=None):
+    """Knobs, all off by default (off, every random draw is the one the plain fuzz makes):
+      gids            an active list, strictly increasing, that may end in ids >= max_groups; position i drives gids[i]
+      leader_share    that fraction of the positions gets only SUBMIT / TIMEOUT ops and in-term replies, so that
+                      groups elected beforehand (elect_all) stay steady-state leaders
+      sweep_every     every k-th row of the stream is a timer sweep row (row_now set), ops and lane events kept
+      stray_requests  every k-th step is flagged RAFTING_INBOX_NO_REQUESTS and keeps its requests
+      t0              added to every time the fuzz writes"""
+
+    def __init__(self, cfg: abi.Cfg, ref, seed=1, rows=3, n=None, gids=None, leader_share=0.0, sweep_every=0,
+                 stray_requests=0, t0=0):
         self.cfg, self.ref = cfg, ref
         self.rng = np.random.default_rng(seed)
+        self.aux = np.random.default_rng([seed, 0xA5])     # the knobs draw from here, never from rng
         self.rows = rows
-        self.n = n or cfg.max_groups
+        self.gids = None if gids is None else np.ascontiguousarray(gids, dtype=np.uint32)
+        if self.gids is not None:
+            assert (np.diff(self.gids.astype(np.int64)) > 0).all(), "active list must be strictly increasing"
+        self.n = len(self.gids) if self.gids is not None else (n or cfg.max_groups)
         self.F = cfg.replicas - 1
-        self.now = T0
-        self.pending = {}      # gid -> list of (lane, kind, inc, epoch, last) replies owed to the SUT
+        self.now = T0 + t0
+        self.pending = {}      # position -> list of (lane, kind, inc, epoch, last) replies owed to the SUT
+        self.steady = np.zeros(self.n, dtype=bool)
+        if leader_share:
+            self.steady[self.aux.permutation(self.n)[:int(leader_share * self.n)]] = True
+        self.sweep_every, self.stray = sweep_every, stray_requests
+        self.row_count = self.step_count = 0
+
+    def gid(self, i: int) -> int:
+        return int(self.gids[i]) if self.gids is not None else i
 
     def _peer(self):
         R = self.cfg.replicas
@@ -97,12 +119,17 @@ class Fuzzer:
         return s if s < self.cfg.local_slot else s + 1
 
     def make(self, last_out: abi.Outbox | None) -> abi.Inbox:
-        rng, F = self.rng, self.F
-        ib = abi.Inbox(self.rows, self.n, F, ent_cap=self.rows * self.n * 8)
-        # harvest reply obligations from the last outbox
+        rng, F, G = self.rng, self.F, self.cfg.max_groups
+        ib = abi.Inbox(self.rows, self.n, F, ent_cap=self.rows * self.n * 8, gids=self.gids, sweep=self.sweep_every > 0)
+        self.step_count += 1
+        if self.stray and self.step_count % self.stray == 0:
+            ib.flags |= abi.INBOX_NO_REQUESTS
+        # harvest reply obligations from the last outbox (a position outside the table has no written cells)
         if last_out is not None:
             for r in range(last_out.rows):
                 for i in range(self.n):
+                    if self.gid(i) >= G:
+                        continue
                     for f in range(F):
                         pm = int(last_out.plan_meta[r, i, f])
                         k = pm & 0xF
@@ -116,9 +143,21 @@ class Fuzzer:
                         for f in range(F):
                             self.pending.setdefault(i, []).append((f, kind, bm >> 32, 0, 0))
         for r in range(self.rows):
+            if self.sweep_every:
+                self.row_count += 1
+                if self.row_count % self.sweep_every == 0:
+                    ib.row_now[r] = self.now + 1
             for i in range(self.n):
                 self.now += 1
-                st = self.ref.export(i)
+                gid = self.gid(i)
+                if gid >= G:               # takes no part in the step; neither side writes its cells
+                    ib.timeout(r, i, self.now)
+                    ib.ack(r, i, 0, self.now, 1, 1, True, 0, 0)
+                    continue
+                st = self.ref.export(gid)
+                if self.steady[i]:
+                    self._steady(ib, r, i, st)
+                    continue
                 term, role = st.current_term, st.role
                 u = rng.random()
                 if u < 0.25:
@@ -141,7 +180,7 @@ class Fuzzer:
                         prev_t = (st.last_term if has else st.epoch_term)
                     elif mode < 0.8 and last > st.epoch_index + 1:   # overlap: rewrite the tail
                         prev = int(rng.integers(st.epoch_index + 1, last))
-                        prev_t = self.ref.log_term(i, prev)
+                        prev_t = self.ref.log_term(gid, prev)
                         if prev_t < 0:
                             prev, prev_t = st.epoch_index, st.epoch_term
                     elif mode < 0.9:     # mismatching prev
@@ -175,7 +214,7 @@ class Fuzzer:
                     has = st.last_index >= st.first_index
                     hi = st.last_index if has else st.epoch_index
                     idx = int(rng.integers(max(st.epoch_index - 1, 0), hi + 2))
-                    t = self.ref.log_term(i, idx)
+                    t = self.ref.log_term(gid, idx)
                     ib.flush(r, i, self.now, idx, t if t >= 0 else max(st.epoch_term, 1))
                 # lane events: answer some owed replies (in order per lane), sometimes forge
                 owed = self.pending.get(i, [])
@@ -199,3 +238,284 @@ class Fuzzer:
                     keep = keep[-4 * F:]
                 self.pending[i] = keep
         return ib
+
+    def _steady(self, ib: abi.Inbox, r: int, i: int, st):
+        """A steady position: SUBMIT / keepAlive ops and replies in the group's own term, nearly all successful."""
+        aux = self.aux
+        u = aux.random()
+        if st.role != ROLE_LEADER:
+            ib.timeout(r, i, self.now, rand=int(aux.integers(900, 1801)))
+        elif u < 0.6:
+            ib.submit(r, i, self.now, count=int(aux.integers(1, 4)))
+        elif u < 0.8:
+            ib.timeout(r, i, self.now)
+        used, keep = set(), []
+        for (f, kind, inc, ep, la) in self.pending.get(i, []):
+            if f in used:
+                keep.append((f, kind, inc, ep, la))
+                continue
+            used.add(f)
+            self.now += 1
+            if kind in (EV_AE_ACK, EV_IS_ACK):
+                ib.ack(r, i, f, self.now, inc, st.current_term, aux.random() < 0.95, ep, la, snapshot=kind == EV_IS_ACK)
+            else:
+                ib.vote_reply(r, i, f, self.now, inc, st.current_term, True, pre=kind == EV_PV_REPLY)
+        self.pending[i] = keep[-4 * self.F:]
+
+
+# ---------------------------------------------------------------------------------------------
+# initial states
+# ---------------------------------------------------------------------------------------------
+E40, T31, T33 = 1 << 40, 1 << 31, 1 << 33
+
+
+def wide_init(G, big=(), terms_mod=7) -> np.ndarray:
+    """Groups in `big` open with a log that starts near 2^40 and a term of at least 2^31."""
+    init = init_array(G, terms=np.arange(G) % terms_mod)
+    big = np.asarray(list(big), dtype=np.int64)
+    if len(big):
+        t = T31 + (big % 5)
+        init["term"][big] = t
+        init["epoch_index"][big] = E40 + big
+        init["epoch_term"][big] = t
+        init["first_index"][big] = E40 + big + 1
+        init["last_index"][big] = E40 + big + 2
+        init["last_term"][big] = t
+        init["commit_index"][big] = E40 + big
+    return init
+
+
+# ---------------------------------------------------------------------------------------------
+# poisoned-outbox driver: both sides step into outboxes whose every byte starts as POISON, so a cell one side writes
+# and the other leaves alone differs even when its right value is 0; cells neither side writes still compare equal
+# ---------------------------------------------------------------------------------------------
+POISON = 0xA5
+
+
+def gcols(ib: abi.Inbox, G: int) -> int:
+    """Entries of a per-group outbox column: n under RAFTING_INBOX_COMPACT_GROUPS, else max_groups."""
+    return ib.n if ib.gids is not None and ib.flags & abi.INBOX_COMPACT_GROUPS else G
+
+
+def poisoned_outbox(ib: abi.Inbox, F: int, G: int, fill=POISON) -> abi.Outbox:
+    out = abi.Outbox(ib.rows, ib.n, F, gcols(ib, G))
+    for name, *_ in abi.Outbox.ROW_COLS + abi.Outbox.GROUP_COLS:
+        getattr(out, name).view(np.uint8).fill(fill)
+    return out
+
+
+class OracleSUT:
+    """The CPU oracle stepping into a poisoned outbox."""
+
+    def __init__(self, cfg: abi.Cfg, fill=POISON, threads=8):
+        from oracle import binding
+        self.cfg, self.F, self.G, self.fill, self.threads = cfg, cfg.replicas - 1, cfg.max_groups, fill, threads
+        self.o = binding.Oracle(cfg)
+
+    def open_bulk(self, first, inits):
+        self.o.open_bulk(first, inits)
+
+    def step(self, ib: abi.Inbox) -> abi.Outbox:
+        return self.o.step(ib, threads=self.threads, out=poisoned_outbox(ib, self.F, self.G, self.fill))
+
+    def export(self, gid):
+        return self.o.export(gid)
+
+    def log_term(self, gid, index):
+        return self.o.log_term(gid, index)
+
+    def export_all(self):
+        return [self.o.export(g) for g in range(self.G)]
+
+
+class EngineSUT:
+    """The CUDA engine stepped through rafting_step_device: inbox and poisoned outbox live in device memory."""
+
+    def __init__(self, cfg: abi.Cfg, fill=POISON):
+        import torch
+        from rafting_b200 import engine
+        self.cfg, self.F, self.G, self.fill = cfg, cfg.replicas - 1, cfg.max_groups, fill
+        self.e = engine.Engine(cfg)
+        self.dev = torch.device("cuda", cfg.device)
+
+    def open_bulk(self, first, inits):
+        self.e.open_bulk(first, inits)
+
+    def step(self, ib: abi.Inbox) -> abi.Outbox:
+        import torch
+        from rafting_b200 import devbatch
+        din = devbatch.DevInbox.from_host(ib, self.dev)
+        dout = devbatch.DevOutbox(ib.rows, ib.n, self.F, gcols(ib, self.G), self.dev, fill=self.fill)
+        torch.cuda.synchronize()
+        self.e.step_device(din.as_c(), dout.as_c())
+        torch.cuda.synchronize()
+        return dout.to_host()
+
+    def export(self, gid):
+        return self.e.export(gid)
+
+    def export_all(self):
+        return self.e.export_bulk(0, self.G)
+
+
+def assert_all_states_equal(ref, sut, F, where=""):
+    for gid, (sa, sb) in enumerate(zip(ref.export_all(), sut.export_all())):
+        if state_bytes(sa, F) != state_bytes(sb, F):
+            da, db = sa.as_dict(), sb.as_dict()
+            raise AssertionError(f"group {gid} state differs {where}: { {k: (da[k], db[k]) for k in da if da[k] != db[k]} }")
+
+
+# ---------------------------------------------------------------------------------------------
+# the fuzz matrix: every kernel and launch mode of launch_step (tests/launch_model.py) under every event kind
+# ---------------------------------------------------------------------------------------------
+@dataclass(frozen=True)
+class FuzzCase:
+    id: str
+    R: int
+    G: int
+    seed: int
+    steps: int = 30
+    cpu_steps: int = 10        # the oracle-on-both-sides rehearsal (tests/test_fuzz_matrix_cpu.py)
+    rows: int = 3
+    local_slot: int = 0
+    pre_vote: bool = True
+    n_active: int = 0          # > 0: an active list of that many positions ...
+    tail: int = 0              # ... of which the last `tail` hold ids >= G
+    compact: bool = False      # RAFTING_INBOX_COMPACT_GROUPS on the active list
+    leader_share: float = 0.0  # > 0: elect every group first, then keep this share steady
+    sweep_every: int = 0
+    stray: int = 0
+    wide: bool = False         # a third of the groups near 2^40 / terms >= 2^31, fuzz times 2^33 ms later
+    state_every: int = 10
+    legacy: bool = False       # a stream the suite has replayed unchanged since before the knobs existed
+
+    @property
+    def n(self):
+        return self.n_active or self.G
+
+    def cfg(self) -> abi.Cfg:
+        return abi.make_cfg(replicas=self.R, local_slot=self.local_slot, max_groups=self.G, max_rows=self.rows,
+                            pre_vote=self.pre_vote, entry_pool_cap=self.rows * self.n * 8)
+
+    def init(self) -> np.ndarray:
+        return wide_init(self.G, range(0, self.G, 3) if self.wide else (), terms_mod=3)
+
+    def gids(self):
+        if not self.n_active:
+            return None
+        pick = np.random.default_rng([self.seed, 0x61D5]).choice(self.G, self.n_active - self.tail, replace=False)
+        return np.concatenate([np.sort(pick), self.G + 3 * np.arange(self.tail)]).astype(np.uint32)
+
+
+def _u(id, R, G, seed, **kw):
+    return FuzzCase(id, R, G, seed, sweep_every=kw.pop("sweep_every", 7), stray=kw.pop("stray", 4), **kw)
+
+
+def _s(id, R, G, seed, **kw):
+    return FuzzCase(id, R, G, seed, steps=kw.pop("steps", 14), cpu_steps=kw.pop("cpu_steps", 8), leader_share=0.35,
+                    sweep_every=kw.pop("sweep_every", 11), stray=kw.pop("stray", 3), state_every=5, **kw)
+
+
+# steps launched without a class sort (n < 2048, a NO_REQUESTS step, or R > 9)
+FUZZ_UNSORTED = [
+    FuzzCase("3-0-True-1", 3, 48, 1, steps=60, legacy=True),
+    FuzzCase("3-2-False-2", 3, 48, 2, steps=60, local_slot=2, pre_vote=False, legacy=True),
+    FuzzCase("5-2-True-3", 5, 48, 3, steps=60, local_slot=2, legacy=True),
+    FuzzCase("4-1-True-4", 4, 48, 4, steps=60, local_slot=1, legacy=True),
+    FuzzCase("7-6-False-5", 7, 48, 5, steps=60, local_slot=6, pre_vote=False, legacy=True),
+    _u("R2-G777", 2, 777, 21, local_slot=1),
+    _u("R2-G777-wide", 2, 777, 22, wide=True),
+    _u("R3-G777", 3, 777, 23, local_slot=1),
+    _u("R3-G777-wide", 3, 777, 24, wide=True, pre_vote=False),
+    _u("R3-n2047", 3, 2047, 25, steps=16),
+    _u("R4-G777-wide", 4, 777, 26, local_slot=3, wide=True),
+    _u("R6-G777", 6, 777, 27, local_slot=2),
+    _u("R6-G777-wide", 6, 777, 28, wide=True),
+    _u("R9-G777", 9, 777, 29, local_slot=8),
+    _u("R9-n2047", 9, 2047, 30, steps=16),
+    _u("R10-G300", 10, 300, 31, local_slot=4),
+    _u("R17-G300-wide", 17, 300, 32, wide=True),
+    _u("R33-G300", 33, 300, 33, local_slot=32, pre_vote=False),
+    _u("R33-G300-wide", 33, 300, 34, wide=True),
+    _u("R3-active1500-compact", 3, 4096, 35, n_active=1500, tail=37, compact=True, steps=16),
+]
+
+# steps that may carry requests over >= 2048 positions at R <= 9: classify_kernel sorts them
+FUZZ_SORTED = [
+    FuzzCase("3-11", 3, 2304, 11, steps=14, cpu_steps=6, local_slot=1, legacy=True),
+    FuzzCase("5-12", 5, 2304, 12, steps=14, cpu_steps=6, local_slot=1, legacy=True),
+    _s("R2-G2304", 2, 2304, 41),
+    _s("R2-G2304-wide", 2, 2304, 42, local_slot=1, wide=True),
+    _s("R3-n2048", 3, 2048, 43, local_slot=2),
+    _s("R3-G2304-wide", 3, 2304, 44, wide=True),
+    _s("R4-G2304-wide", 4, 2304, 45, local_slot=1, wide=True),
+    _s("R6-G2304", 6, 2304, 46, local_slot=5),
+    _s("R9-G2304-wide", 9, 2304, 47, local_slot=3, wide=True),
+    _s("R9-n2048", 9, 2048, 48),
+    _s("R3-active2100", 3, 4096, 49, n_active=2100, tail=40),
+    _s("R5-active2100-compact", 5, 4096, 50, n_active=2100, tail=40, compact=True),
+    _s("R9-active2100-compact", 9, 4096, 51, n_active=2100, tail=40, compact=True),
+]
+
+
+@dataclass
+class Coverage:
+    roles: set = field(default_factory=set)
+    errs: set = field(default_factory=set)
+    classes: list = field(default_factory=list)     # per class-sorted step: positions per class
+    launches: set = field(default_factory=set)      # (kernels, mode) of launch_model.kernels
+
+
+def run_fuzz_case(case: FuzzCase, sut_factory, steps=None, ref_factory=OracleSUT) -> Coverage:
+    """Drives `case` through a poisoned reference (the oracle) and a poisoned SUT, comparing every outbox, the state of a
+    spread of groups every `state_every` steps and of every group at the end."""
+    from tests import launch_model
+    cfg, F, G = case.cfg(), case.R - 1, case.G
+    ref, sut = ref_factory(cfg), sut_factory(cfg)
+    init = case.init()
+    ref.open_bulk(0, init)
+    sut.open_bulk(0, init)
+    out = None
+    if case.leader_share:
+        w1 = workload.make_wl(case.seed, 1, G, F, local_slot=case.local_slot)
+        out = elect_all(ref, w1)
+        assert_outbox_equal(out, elect_all(sut, w1), where=f"{case.id}: election")
+    gids = case.gids()
+    fz = Fuzzer(cfg, ref, seed=case.seed, rows=case.rows, gids=gids, leader_share=case.leader_share,
+                sweep_every=case.sweep_every, stray_requests=case.stray, t0=T33 if case.wide else 0)
+    # the cells a step writes for certain: the group columns of the groups that take part, the rows of their positions
+    pos = np.arange(fz.n) if gids is None else np.flatnonzero(gids < G)
+    grp = pos if gids is None or case.compact else gids[pos]
+    spread = np.arange(0, G, max(1, G // 97))
+    if gids is not None:
+        spread = np.union1d(spread, gids[pos][:64])
+    cov = Coverage()
+    for k in range(case.steps if steps is None else steps):
+        ib = fz.make(out)
+        if case.compact:
+            ib.flags |= abi.INBOX_COMPACT_GROUPS
+        launch = launch_model.kernels(case.R, ib.n, ib.flags)
+        cov.launches.add(launch)
+        if launch[1] == "class-sorted":
+            cov.classes.append(np.bincount(launch_model.classes(ref, ib), minlength=launch_model.NCLS))
+        out = ref.step(ib)
+        assert_outbox_equal(out, sut.step(ib), where=f"{case.id}: fuzz step {k}")
+        cov.roles |= set((out.role_word[grp] & 3).tolist())
+        cov.errs |= set(((out.rep_meta[:, pos] >> 8) & 0xFF).ravel().tolist())
+        if k % case.state_every == case.state_every - 1:
+            assert_states_equal(ref, sut, spread.tolist(), F, where=f"{case.id}: fuzz step {k}")
+    assert_all_states_equal(ref, sut, F, where=f"{case.id}: end of the fuzz")
+    return cov
+
+
+def check_coverage(case: FuzzCase, cov: Coverage):
+    """The steering reached what the case is there for: every role, several error paths and, in a class-sorted case
+    whose leaders are steered, every class most of the time and the two leader classes each wider than a 128-thread
+    block in some step."""
+    assert cov.roles == {0, 1, 2}, cov.roles
+    assert len(cov.errs) > 3, cov.errs
+    if case.leader_share:
+        c = np.array(cov.classes)
+        assert len(c), "no class-sorted step"
+        assert ((c > 0).all(axis=1)).mean() > 0.5, c.tolist()
+        assert c[:, 2].max() > 128 and c[:, 3].max() > 128, c.tolist()

@@ -589,6 +589,36 @@ def test_install_snapshot_request():
     assert rep(out) == (1, 0, 0, t)
 
 
+def test_requests_refused_in_a_step_promising_none():
+    """rafting_b200.h, RAFTING_INBOX_NO_REQUESTS: a step flagged to hold no inbound requests answers any request op
+    found anyway with BAD_EVENT and an invalid reply, and leaves term, ballot, timer and log as they were.  SUBMIT and
+    TIMEOUT still run in such a step."""
+    g = One(term=3, ballot=1, first_index=1, last_index=5, last_term=3)
+    g.timeout()                                            # timeoutDetected: a pre-vote would otherwise be granted
+    before = g.st
+    requests = [
+        lambda ib: ib.ae_request(0, 0, g.now, 2, 7, 5, 3, [7, 7], leader_commit=6, rand=1300),
+        lambda ib: ib.prevote_request(0, 0, g.now, 2, 4, 9, 3, rand=1300),
+        lambda ib: ib.vote_request(0, 0, g.now, 2, 8, 9, 3, rand=1300),
+        lambda ib: ib.is_request(0, 0, g.now, 2, 9, 40, 3, True, rand=1300),
+        lambda ib: ib.flush(0, 0, g.now, 2, 3),
+    ]
+    for k, put in enumerate(requests):
+        ib = g.inbox(); put(ib); ib.flags = abi.INBOX_NO_REQUESTS
+        out = g.run(ib)
+        assert rep(out)[:3] == (0, 0, ERR["BAD_EVENT"]), k
+        s = g.st
+        assert err_code(s.err_word) == ERR["BAD_EVENT"] and s.err_word >> 16 == k + 1
+        for name in ("role", "current_term", "voted_for", "current_leader", "incarnation", "timer", "commit_index",
+                     "epoch_index", "first_index", "last_index", "last_term", "log_digest"):
+            assert getattr(s, name) == getattr(before, name), (k, name)
+        assert int(out.current_term[0]) == 3 and int(out.ballot_meta[0, 0]) == 0
+    g.now += 10
+    ib = g.inbox(); ib.timeout(0, 0, g.now, rand=1200); ib.flags = abi.INBOX_NO_REQUESTS
+    out = g.run(ib)
+    assert rep(out)[2] == 0 and int(out.ballot_meta[0, 0]) & 0xF == abi.BALLOT_PREVOTE and g.st.timer == g.now + 1200
+
+
 def test_restart_over_a_log_with_several_terms():
     """RaftContext.initialize over an existing RocksLog (RaftContext.java:91-113): the index->term map of the stored log
     comes back as runs; AppendEntries consistency checks must then see the right term at every index."""

@@ -4,7 +4,6 @@ Indices near 2^40, terms of 2^31 and more, a failure stamped more than 2^31 ms i
 index jump by 2^31 in the middle of a launch, recovery_cool_down_ms > 0 with no failure yet, warps that mix such groups
 with ordinary ones, and a partial last block.  Every outbox column and the exported state must stay bit-exact.  All tests
 need an H100 (`-m gpu`)."""
-import numpy as np
 import pytest
 
 from oracle import binding
@@ -13,8 +12,7 @@ from tests import harness
 
 pytestmark = pytest.mark.gpu
 
-E40 = 1 << 40
-T31 = 1 << 31
+E40, T31 = harness.E40, harness.T31
 
 
 @pytest.fixture(scope="module")
@@ -24,26 +22,10 @@ def engine_mod():
     return engine
 
 
-def _init(G, big=()):
-    """Groups in `big` open with a log that starts near 2^40 and a term of at least 2^31."""
-    init = harness.init_array(G, terms=np.arange(G) % 7)
-    big = np.asarray(list(big), dtype=np.int64)
-    if len(big):
-        t = T31 + (big % 5)
-        init["term"][big] = t
-        init["epoch_index"][big] = E40 + big
-        init["epoch_term"][big] = t
-        init["first_index"][big] = E40 + big + 1
-        init["last_index"][big] = E40 + big + 2
-        init["last_term"][big] = t
-        init["commit_index"][big] = E40 + big
-    return init
-
-
 def _run(sut_factory, G, rows, steps=10, big=(), mutate=None, **cfgkw):
     cfg = abi.make_cfg(replicas=3, max_groups=G, max_rows=rows, **cfgkw)
     o, e = binding.Oracle(cfg), sut_factory(cfg)
-    init = _init(G, big)
+    init = harness.wide_init(G, big)
     o.open_bulk(0, init)
     e.open_bulk(0, init)
     w1 = workload.make_wl(0x5EED0032, 1, G, 2)

@@ -12,14 +12,6 @@ from tests import harness
 pytestmark = pytest.mark.gpu
 
 
-def _to_host(dob, rows, n, F, G) -> abi.Outbox:
-    o = abi.Outbox(rows, n, F, G)
-    for name, t in dob.t.items():
-        a = getattr(o, name)
-        a[...] = np.frombuffer(t.cpu().numpy().tobytes(), dtype=a.dtype).reshape(a.shape)
-    return o
-
-
 @pytest.mark.parametrize("G,rows,launches", [(1024, 8, 12), (777, 5, 9)])
 def test_device_sequence_matches_oracle(G, rows, launches):
     import torch
@@ -50,5 +42,5 @@ def test_device_sequence_matches_oracle(G, rows, launches):
     e.step_device_seq(ics, ocs, launches)
     torch.cuda.synchronize()
     for k in range(launches):
-        harness.assert_outbox_equal(want[k], _to_host(douts[k], rows, G, F, G), where=f"launch {k} of the sequence")
+        harness.assert_outbox_equal(want[k], douts[k].to_host(), where=f"launch {k} of the sequence")
     harness.assert_states_equal(o, e, range(G), F, where="end of the sequence")
