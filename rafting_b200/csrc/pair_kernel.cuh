@@ -38,15 +38,55 @@ struct __align__(16) PStage {            // one staged input row of a block (TPB
     uint64_t ev_meta[PTPB];
 };
 
+// The group scalars the fast path only reads — only the generic handler (slow_row) changes them: one copy per group slot
+// in shared memory rather than a register copy in each lane of the pair, which at the 64-register cap one wave needs
+// pushed the row loop's state into local memory.  Lane 0 fills its slot from the tables after every (re)load, and a pair
+// __syncwarp publishes it to lane 1.  GS's copies of these fields are not read inside the row loop.
+struct PSlab {
+    int64_t  term[TPB], lo[TPB], epochIndex[TPB], epochTerm[TPB], r0s[TPB], r0t[TPB];
+    uint32_t inc[TPB];
+};
+__device__ __forceinline__ void load_slab(const Tables& T, uint32_t gid, PSlab& s, uint32_t tl) {
+    s.inc[tl] = (uint32_t)(__ldcg(T.g_meta + gid) >> 32);
+    s.term[tl] = __ldcg(T.g_term + gid); s.lo[tl] = __ldcg(T.g_lo + gid);
+    const longlong2 ep = __ldcg((const longlong2*)(T.g_epoch + gid)); s.epochIndex[tl] = ep.x; s.epochTerm[tl] = ep.y;
+    const longlong2 r0 = __ldcg((const longlong2*)(T.g_runs + gid)); s.r0s[tl] = r0.x; s.r0t[tl] = r0.y;
+}
+__device__ __forceinline__ void slab_to_gs(const PSlab& s, uint32_t tl, GS& g) {
+    g.inc = s.inc[tl]; g.term = s.term[tl]; g.lo = s.lo[tl];
+    g.epochIndex = s.epochIndex[tl]; g.epochTerm = s.epochTerm[tl]; g.r0s = s.r0s[tl]; g.r0t = s.r0t[tl];
+}
+
+// v, through an empty asm the compiler cannot move out of the row loop: the table addresses the rare hand-off to slow_row
+// derives from it are computed where they are used, not hoisted and carried (in local memory) around the loop
+__device__ __forceinline__ uint32_t in_place(uint32_t v) { asm volatile("" : "+r"(v)); return v; }
+
+// term_at for an index outside the newest term run: the walk over the older runs.  Rare on the leader stream (a commit
+// index below the newest run), and out of line so that the run table's address is not carried across the ack path.
+// .x: found, .y: the term
+__device__ __noinline__ i64x2 term_at_older(const i64x2* runs, uint32_t G, uint32_t word, int64_t lo, int64_t hi,
+                                            int64_t r0s, int64_t r0t, int64_t idx) {
+    GS g; g.word = word; g.lo = lo; g.hi = hi; g.r0s = r0s; g.r0t = r0t;
+    Ctx c; c.runs = const_cast<i64x2*>(runs); c.G = G;
+    int64_t t = 0;
+    const bool found = term_at(g, c, idx, t);
+    i64x2 v; v.x = found; v.y = t;
+    return v;
+}
+
 // tryCommit for R = 3 on explicit matchIndex values (Leader.java:247-280, Leadership.java:116-130: sorted[F/2] of two
 // values is the larger one, sorted[0] the smaller)
-__device__ __forceinline__ void try_commit2(GS& g, const Ctx& c, int64_t ma, int64_t mb) {
+__device__ __forceinline__ void try_commit2(GS& g, const PSlab& s, uint32_t tl, const Tables& T, uint32_t gid, int64_t ma, int64_t mb) {
     const int64_t full = ma < mb ? ma : mb, major = ma < mb ? mb : ma;
     if (major == 0) return;
     int64_t t;
-    if (nruns_of(g) > 0 && major >= g.r0s && major <= g.hi) t = g.r0t;
-    else if (!term_at(g, c, major, t)) { flag_err(g, RAFTING_ERR_TRY_COMMIT_FAILED); return; }
-    const int64_t ci = (t == g.term) ? major : full;
+    if (nruns_of(g) > 0 && major >= s.r0s[tl] && major <= g.hi) t = s.r0t[tl];
+    else {
+        const i64x2 v = term_at_older(T.g_runs + gid, T.G, g.word, s.lo[tl], g.hi, s.r0s[tl], s.r0t[tl], major);
+        if (!v.x) { flag_err(g, RAFTING_ERR_TRY_COMMIT_FAILED); return; }
+        t = v.y;
+    }
+    const int64_t ci = (t == s.term[tl]) ? major : full;
     if (ci != 0 && ci != g.commit) { const int e = commit_log(g, ci); if (e) flag_err(g, e); }
 }
 
@@ -55,6 +95,7 @@ __global__ void __launch_bounds__(PTPB, RAFTING_PAIR_MINBLOCKS)
 pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, CfgD cfg) {
     static_assert(NST >= 2, "the ring needs at least two stages");
     __shared__ KArgs ka;
+    __shared__ PSlab slab;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     PStage* stage = reinterpret_cast<PStage*>(smem_raw);
     // a programmatic launch behind this one (launch_pair) may start its blocks as soon as these exit
@@ -97,8 +138,9 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
     // the inbox is read-only here and written by no step kernel; the tables and the outbox are the previous launch's: wait
     // for it (a no-op unless this is a programmatic launch)
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    GS g; LS x;
-    load_hot(T, gid, g); g.dirty = 0; g.electTerm = 0; g.electInc = 0; g.votes = 0;
+    if (f == 0) load_slab(T, gid, slab, tl);   // published by the row loop's first __syncwarp
+    GS g; LS x;                                 // of GS only word, commit, hi, timer, err and dirty are live in the row loop
+    load_hot(T, gid, g); g.dirty = 0;
     if (!valid) g.word = 0;
     load_lane(T, li, x);
 
@@ -129,7 +171,7 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
             const bool unav = hasAb && (((uint64_t)st.op_ab[tl].x >> f) & 1ull) != 0;
             kind = RAFTING_OP_KIND(meta);
             const bool submit = kind == RAFTING_OP_SUBMIT, hb = kind == RAFTING_OP_TIMEOUT;
-            const bool fastOk = leaderLive && (hb || (submit && nruns_of(g) > 0 && g.r0t == g.term));
+            const bool fastOk = leaderLive && (hb || (submit && nruns_of(g) > 0 && slab.r0t[tl] == slab.term[tl]));
             // Leader.isReady (Leader.java:52-64) needs every follower's State: one ballot
             const bool myReady = state_ready(x, cfg.avail_critical_point, cfg.recovery_cool_down_ms, now);
             const uint32_t rb = (__ballot_sync(0xffffffffu, myReady) >> (lane & ~1u)) & 3u;
@@ -148,7 +190,7 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
             if (unav) cls = 4;
             else if (x.inflight > limit) cls = 3;
             else if (x.pending) cls = 2;
-            else cls = (nruns_of(g) > 0 && p > g.epochIndex && p >= g.r0s && p >= g.lo && p <= hiNew) ? 1 : 0;
+            else cls = (nruns_of(g) > 0 && p > slab.epochIndex[tl] && p >= slab.r0s[tl] && p >= slab.lo[tl] && p <= hiNew) ? 1 : 0;
             const uint32_t gb = (__ballot_sync(0xffffffffu, cls != 0) >> (lane & ~1u)) & 3u;
             if (kind != RAFTING_OP_NONE) {
                 if (!fastOk || (ready && gb != 3u)) slowOp = true;      // the generic handler takes the whole row
@@ -158,16 +200,16 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
                 } else {
                     if (submit) { g.word |= W_READY; g.hi = hiNew; }
                     else g.timer = (I64MAX - cfg.heartbeat_ms < now) ? I64MAX : now + cfg.heartbeat_ms;   // resetTimer, Leader branch
-                    const uint64_t hbit = hb ? (1ull << 4) : 0ull, incBits = (uint64_t)g.inc << 32;
+                    const uint64_t hbit = hb ? (1ull << 4) : 0ull, incBits = (uint64_t)slab.inc[tl] << 32;
                     if (now > x.lastReq) x.lastReq = now;               // :158
                     if (cls == 4) { stat_failure(x, now, true, false); pm = RAFTING_PLAN_UNAVAILABLE | hbit | incBits; }
                     else if (cls == 3) pm = RAFTING_PLAN_SKIP_INFLIGHT | hbit | incBits;
                     else if (cls == 2) {
-                        pm = RAFTING_PLAN_IS | hbit | incBits; p0 = g.epochIndex; p1 = g.epochTerm; l0 = g.epochIndex; l1 = g.commit;
+                        pm = RAFTING_PLAN_IS | hbit | incBits; p0 = slab.epochIndex[tl]; p1 = slab.epochTerm[tl]; l0 = p0; l1 = g.commit;
                         x.inflight++;
                     } else {
                         const int64_t lastIdx = (g.hi - p > (int64_t)fetch) ? p + fetch : g.hi;
-                        pm = RAFTING_PLAN_AE | hbit | ((uint64_t)(lastIdx - p) << 16) | incBits; p0 = p; p1 = g.r0t; l0 = lastIdx; l1 = g.commit;
+                        pm = RAFTING_PLAN_AE | hbit | ((uint64_t)(lastIdx - p) << 16) | incBits; p0 = p; p1 = slab.r0t[tl]; l0 = lastIdx; l1 = g.commit;
                         x.inflight++;
                     }
                 }
@@ -176,23 +218,26 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
         if (slowOp) {
             // ---- the generic handler takes the whole row (op + events): state goes through the tables (pair-uniform) ----
             const uint32_t pmask = 3u << (lane & ~1u);
+            const uint32_t hg = in_place(gid);
+            const size_t hl = (size_t)hg * 2u + f;
             if (valid) {
-                store_lane(T, li, x);
-                if (f == 0) { store_hot(T, gid, g); if (out.ballot_meta) out.ballot_meta[gi] = 0; }
+                store_lane(T, hl, x);
+                if (f == 0) { g.inc = slab.inc[tl]; store_hot(T, hg, g); if (out.ballot_meta) out.ballot_meta[gi] = 0; }
             }
             __syncwarp(pmask);
             uint32_t dirty = g.dirty;
-            if (valid && f == 0) dirty = slow_row<2>(&ka, i, gid, r, kind, sweep, 1u | (hasEv ? 2u : 0u), 0u, g.dirty);
+            if (valid && f == 0) dirty = slow_row<2>(&ka, i, hg, r, kind, sweep, 1u | (hasEv ? 2u : 0u), 0u, g.dirty);
+            if (f == 0) load_slab(T, hg, slab, tl);
             __syncwarp(pmask);
             dirty = __shfl_sync(pmask, dirty, lane & ~1u);
-            load_hot(T, gid, g); g.dirty = dirty; if (!valid) g.word = 0;
-            load_lane(T, li, x);
+            load_hot(T, hg, g); g.dirty = dirty; if (!valid) g.word = 0;
+            load_lane(T, hl, x);
             handled = true;
         } else if (valid) {
             if (out.plan_meta) {
                 const size_t pl = (size_t)gi * 2u + f;
                 out.plan_meta[pl] = pm;
-                if (pm != 0) { i64x2 v; v.x = p0; v.y = p1; out.plan_pp[pl] = v; v.x = l0; v.y = l1; out.plan_lc[pl] = v; out.plan_epoch[pl] = g.epochIndex; }
+                if (pm != 0) { i64x2 v; v.x = p0; v.y = p1; out.plan_pp[pl] = v; v.x = l0; v.y = l1; out.plan_lc[pl] = v; out.plan_epoch[pl] = slab.epochIndex[tl]; }
             }
             if (f == 0) { if (out.rep_meta) out.rep_meta[gi] = repMeta; if (out.ballot_meta) out.ballot_meta[gi] = 0; }
         }
@@ -205,10 +250,10 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
             if (ek != RAFTING_EV_NONE) { etn = st.ev_tn[tid]; if (hasEl) eel = st.ev_el[tid]; }
             const bool ok = RAFTING_EVM_OUTCOME(em) == RAFTING_OUT_OK, snap = ek == RAFTING_EV_IS_ACK;
             const bool isAck = ek == RAFTING_EV_AE_ACK || ek == RAFTING_EV_IS_ACK;
-            const bool mine = isAck && leaderLive && RAFTING_EVM_INC(em) == g.inc;   // addressed to the live Leadership.State
+            const bool mine = isAck && leaderLive && RAFTING_EVM_INC(em) == slab.inc[tl];   // addressed to the live Leadership.State
             // what the serial loop hands to the generic handler "from this lane on": other kinds, a higher term
             // (Leader.java:178-180,224-226), a matchIndex rollback (Leadership.java:76-81)
-            const bool bail = alive && (ek > RAFTING_EV_IS_ACK || (mine && ok && (etn.x > g.term || (snap ? eel.x : eel.y) < x.match)));
+            const bool bail = alive && (ek > RAFTING_EV_IS_ACK || (mine && ok && (etn.x > slab.term[tl] || (snap ? eel.x : eel.y) < x.match)));
             const uint32_t bb = (__ballot_sync(0xffffffffu, bail) >> (lane & ~1u)) & 3u;
             const uint32_t bailAt = bb == 0 ? 2u : (uint32_t)(__ffs((int)bb) - 1);
             const int64_t mo = x.match;
@@ -235,22 +280,24 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
             const int64_t mn = x.match;
             const int64_t peerOld = __shfl_xor_sync(0xffffffffu, mo, 1), peerNew = __shfl_xor_sync(0xffffffffu, mn, 1);
             if (tb) {
-                const Ctx c = make_ctx(T, cfgp, gid, 0, 0);
                 const int64_t m0n = f == 0 ? mn : peerNew, m1o = f == 0 ? peerOld : mo, m1n = f == 0 ? peerNew : mn;
-                if (tb & 1u) try_commit2(g, c, m0n, m1o);
-                if (tb & 2u) try_commit2(g, c, m0n, m1n);
+                if (tb & 1u) try_commit2(g, slab, tl, T, gid, m0n, m1o);
+                if (tb & 2u) try_commit2(g, slab, tl, T, gid, m0n, m1n);
             }
             if (bailAt < 2u) {
                 // pair-uniform: the generic handler finishes this row from lane bailAt on
                 const uint32_t pmask = 3u << (lane & ~1u);
-                if (valid) { store_lane(T, li, x); if (f == 0) store_hot(T, gid, g); }
+                const uint32_t hg = in_place(gid);
+                const size_t hl = (size_t)hg * 2u + f;
+                if (valid) { store_lane(T, hl, x); if (f == 0) { g.inc = slab.inc[tl]; store_hot(T, hg, g); } }
                 __syncwarp(pmask);
                 uint32_t dirty = g.dirty;
-                if (valid && f == 0) dirty = slow_row<2>(&ka, i, gid, r, 0u, 0, 2u, bailAt, g.dirty);
+                if (valid && f == 0) dirty = slow_row<2>(&ka, i, hg, r, 0u, 0, 2u, bailAt, g.dirty);
+                if (f == 0) load_slab(T, hg, slab, tl);
                 __syncwarp(pmask);
                 dirty = __shfl_sync(pmask, dirty, lane & ~1u);
-                load_hot(T, gid, g); g.dirty = dirty; if (!valid) g.word = 0;
-                load_lane(T, li, x);
+                load_hot(T, hg, g); g.dirty = dirty; if (!valid) g.word = 0;
+                load_lane(T, hl, x);
             }
         }
     }
@@ -258,7 +305,7 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
     if (!valid) return;
     // ---- write back: lane f its Leadership.State, lane 0 the group columns the fast path can change ----
     store_lane(T, li, x);
-    if (f == 0) { store_hot(T, gid, g); write_group_columns(in, out, i, gid, g); }
+    if (f == 0) { slab_to_gs(slab, tl, g); store_hot(T, gid, g); write_group_columns(in, out, i, gid, g); }
 #undef PAIR_ISSUE
 }
 
