@@ -415,7 +415,8 @@ int rafting_step_wait_slot (rafting_engine_t* e, uint32_t slot);
  *     slot 0..31 of its (group, follower) lane), the reply echoes the tag, unpack looks the pair up and frees the slot.
  *     No free slot (more than 32 RPCs of one lane outstanding): tag 255, and the reply must come back as an escape record.
  *   * dense steps only (no active list).  op_c carries SUBMIT / TIMEOUT ops, ev_c AE / IS acks; vote replies and anything
- *     irregular use the escape lists.  Inbound requests ride beside the inbox in a request list (rafting_creqs_t, below):
+ *     irregular use the escape lists (vote replies, ballots and vote requests travel compact under RAFTING_COMPACT_ELECTIONS,
+ *     below).  Inbound requests ride beside the inbox in a request list (rafting_creqs_t, below):
  *     AppendEntries as 32-byte records, every other request kind as an op escape.  A step without requests runs as
  *     RAFTING_INBOX_NO_REQUESTS.
  *   * wire words are 32 bits: 4 B per lane slot + 4 B per group row up, 4 B per lane slot + 1 B per group row down.
@@ -550,6 +551,44 @@ int rafting_compact_req_layout(uint32_t n_req, uint32_t n_op_esc, uint32_t ent_c
    an empty one) rep_c carries compact replies.  rafting_step_wait_compact / rafting_step_fetch_dense serve both. */
 int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot /* 0..3 */, const rafting_cinbox_t* in_host,
                                    const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host);
+/* ELECTIONS on the compact path (flag RAFTING_COMPACT_ELECTIONS of rafting_step_begin_compact_ex; flags == 0 is exactly
+ * rafting_step_begin_compact_req).  Election traffic comes in storms (a node restarts, a partition heals, every group that
+ * had its leader there elects at once); under the flag a ballot, its replies and inbound vote requests travel compact too.
+ *   * ballot (down): a PreVote / RequestVote broadcast of (row, group) becomes one plan_c word per lane of the group, kind
+ *     RAFTING_CPLAN_PREVOTE (5) / RAFTING_CPLAN_VOTE (6), a tag in bits 5..10 (63 = none), no payload.  It stands for
+ *          ballot_meta = BALLOT_PREVOTE / BALLOT_VOTE | incarnation[g] << 32, ballot_term = current_term[g] + 1 (PreVote) /
+ *          current_term[g] (RequestVote), ballot_last = last_entry[g]      (end-of-step columns, as for plans)
+ *     and is used only when exactly that holds and no lane of the (row, group) also holds a plan; every other ballot stays a
+ *     RAFTING_CESC_BALLOT escape record and takes no tag.  counts[1] counts both.  Each lane's word takes the lowest free tag
+ *     of its lane and parks (ballot term, 0) and the incarnation under it: a vote RPC completes exactly once, like an AE / IS.
+ *   * vote reply (up), an ev_c word of kind RAFTING_EV_PV_REPLY / RAFTING_EV_RV_REPLY:
+ *        bits 0..3 kind | 4..5 outcome | 6 granted | 7 reserved (0) | 8..12 tag (0..31) | 13..15 c | 16..31 now - row_base[row]
+ *        Bit 7 is reserved: a writer sets it to 0, and unpack ignores it (it does not reach ev_meta; unlike an ack word, a vote
+ *        word has no term-as-sent bit, the term comes from c).
+ *        The step sees: the incarnation and ballot term parked under the tag (the tag is freed), respTerm = ballotTerm - c for
+ *        outcome OK and 0 otherwise (c must then be 0), ev_el = (0, 0).  A reply with no tag, respTerm > ballotTerm,
+ *        ballotTerm - respTerm > 7, a non-zero respTerm without outcome OK, or a time out of range is an escape record.
+ *   * escaped word: RAFTING_CEV_ESCAPED | tag << 8 carries the tag of the RPC the escaped event answers (any value >= 32 = none);
+ *     unpack frees it, so escaped replies (AE / IS acks included) do not leak tags.  Unflagged steps ignore bits 8..31.
+ *   * vote record (rafting_creq_t, request list): meta bits 11..12 = 1 PreVote / 2 RequestVote (RAFTING_CREQ_VOTE_*),
+ *        prev_index = lastLogIndex, d_prev_term = term - lastLogTerm, entry count 0, d_commit 0.  The step sees kind
+ *        PREVOTE_REQ / VOTE_REQ, a = term, b = prev_index, c = term - d_prev_term, d = e = 0, entry offset 0.  A vote record
+ *        with a non-zero count or d_commit, or bits 11..12 == 3, is malformed, like a record with bits 13..15 set.  Without
+ *        the flag any non-zero bit 11..15 stays malformed.
+ *   Replies to inbound vote requests need nothing new: rep_c bit 7 already covers a valid reply with the end-of-step term. */
+#define RAFTING_COMPACT_ELECTIONS 1u
+#define RAFTING_CPLAN_PREVOTE 5u
+#define RAFTING_CPLAN_VOTE    6u
+#define RAFTING_CEV_VOTE_MAKE(kind, outcome, granted, tag, c, dt)                                                      \
+    ((uint32_t)(kind) | ((uint32_t)(outcome) << 4) | ((uint32_t)((granted) ? 1 : 0) << 6) | ((uint32_t)((tag) & 0x1fu) << 8) | \
+     ((uint32_t)((c) & 7u) << 13) | ((uint32_t)((dt) & 0xffffu) << 16))
+#define RAFTING_CEV_VOTE_TAG(w)  (((uint32_t)(w) >> 8) & 0x1fu)
+#define RAFTING_CEV_VOTE_C(w)    (((uint32_t)(w) >> 13) & 7u)
+#define RAFTING_CREQ_VOTE_PRE 1u
+#define RAFTING_CREQ_VOTE_RV  2u
+#define RAFTING_CREQ_VOTE(m)  (((uint32_t)(m) >> 11) & 3u)
+int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot /* 0..3 */, const rafting_cinbox_t* in_host,
+                                  const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host, uint32_t flags);
 int rafting_step_wait_compact (rafting_engine_t* e, uint32_t slot);
 /* the dense outbox of the compact step last waited for in `slot` (every column that is non-NULL in out_host): the lossless
    fallback when the escape list overflowed */

@@ -230,6 +230,25 @@ int rafting_failures_to_cinbox(rafting_pending_t* p, uint32_t peer, const int32_
                                uint32_t row, const rafting_cinbox_t* cin, uint32_t n_groups, uint32_t F, rafting_cesc_in_t* esc,
                                uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred, uint32_t* n_deferred, uint32_t* n_unknown);
 
+/* The same three writers for a step begun with RAFTING_COMPACT_ELECTIONS (rafting_step_begin_compact_ex); flags == 0 is exactly
+ * the function without _ex.  Under the flag:
+ *   rafting_request_to_creq_ex  a PreVote / RequestVote with src_slot < 32, 0 <= now - row_base[row] <= 65535 and
+ *                               0 <= term - lastLogTerm < 2^32 becomes a vote record (no entries, d_commit 0)
+ *   rafting_acks_to_cinbox_ex   a vote reply whose pending entry has a tag (the ballot lane's, put with term = the ballot
+ *                               term) and whose term lies 0..7 below the ballot term becomes a vote word
+ *   rafting_failures_to_cinbox_ex   a timed-out / cancelled vote RPC with a tag becomes a vote word (c = 0)
+ * and every escaped word carries the tag of its pending entry (RAFTING_CEV_ESCAPED | tag << 8), which unpack frees. */
+int rafting_request_to_creq_ex(const rafting_req_rec_t* r, const int64_t* entry_terms, uint32_t row, int64_t now_ms, int host_result,
+                               const rafting_cinbox_t* in, uint32_t n_groups, rafting_creqs_t* q, uint32_t req_cap, uint32_t esc_cap,
+                               uint32_t ent_cap, uint32_t flags);
+int rafting_acks_to_cinbox_ex(rafting_pending_t* p, uint32_t peer, const rafting_ack_rec_t* acks, uint32_t n, int64_t now_ms, uint32_t row,
+                              const rafting_cinbox_t* cin, uint32_t n_groups, uint32_t F, rafting_cesc_in_t* esc, uint32_t esc_cap,
+                              uint32_t* n_esc, uint32_t* deferred, uint32_t* n_deferred, uint32_t* n_unknown, uint32_t flags);
+int rafting_failures_to_cinbox_ex(rafting_pending_t* p, uint32_t peer, const int32_t* sequences, uint32_t n, uint32_t outcome,
+                                  int64_t now_ms, uint32_t row, const rafting_cinbox_t* cin, uint32_t n_groups, uint32_t F,
+                                  rafting_cesc_in_t* esc, uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred, uint32_t* n_deferred,
+                                  uint32_t* n_unknown, uint32_t flags);
+
 /* ---- the inbox builder: what the event loops' queues become (dense / leased path) -------------------------------------------
  * The reference queues work per context on its event loop (EventLoop.java:87-101): replies hop back with execute(urgent),
  * inbound requests and RaftStub.submit are queued behind them.  The builder keeps one FIFO per group — requests (records +

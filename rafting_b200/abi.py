@@ -355,6 +355,17 @@ def creq_make(peer: int, count: int, dt: int) -> int:
     return (peer & 0x1F) | ((count & 0x3F) << 5) | ((dt & 0xFFFF) << 16)
 
 
+# elections on the compact path (rafting_step_begin_compact_ex flag): ballots as plan_c lanes, vote replies as ev_c words,
+# vote requests as records, escaped words carrying the tag they free
+COMPACT_ELECTIONS = 1
+CPLAN_PREVOTE, CPLAN_VOTE = 5, 6
+CREQ_VOTE_PRE, CREQ_VOTE_RV = 1, 2
+
+
+def cev_vote_make(kind: int, outcome: int, granted: int, tag: int, c: int, dt: int) -> int:
+    return kind | (outcome << 4) | ((1 if granted else 0) << 6) | ((tag & 0x1F) << 8) | ((c & 7) << 13) | ((dt & 0xFFFF) << 16)
+
+
 class CReqsC(C.Structure):
     _fields_ = [("n_req", C.c_uint32), ("n_op_esc", C.c_uint32), ("req", C.c_void_p), ("op_esc", C.c_void_p),
                 ("ent_terms", C.c_void_p), ("ent_count", C.c_uint32), ("req_entries", C.c_uint32)]

@@ -89,9 +89,23 @@ class CompactOutbox:
         c.esc, c.esc_cap, c.counts = self.esc.ctypes.data, self.esc_cap, self.counts.ctypes.data
         return c
 
-    def tags(self) -> np.ndarray:
-        """tag of every plan, [rows, n, F] (abi.CTAG_NONE = none)"""
-        return ((self.plan_c >> np.uint32(5)) & np.uint32(63)).astype(np.uint8)
+    def tags(self, rpc_only: bool = False) -> np.ndarray:
+        """tag of every plan, [rows, n, F] (abi.CTAG_NONE = none).  rpc_only: CTAG_NONE on every lane that holds no AE / IS
+        plan, so that every tag names an AppendEntries / InstallSnapshot in flight (what encode_inbox(elections=True) needs
+        for acks: its escaped words free their tag)."""
+        t = ((self.plan_c >> np.uint32(5)) & np.uint32(63)).astype(np.uint8)
+        if rpc_only:
+            k = self.plan_c & np.uint32(7)
+            t[(k != abi.PLAN_AE) & (k != abi.PLAN_IS)] = abi.CTAG_NONE
+        return t
+
+    def ballot_tags(self) -> np.ndarray:
+        """tag of every compact ballot lane of a step begun with abi.COMPACT_ELECTIONS, [rows, n, F]; CTAG_NONE on every other
+        lane (an escaped ballot takes no tag, and a lane's AE / IS tag never answers a vote)"""
+        t = ((self.plan_c >> np.uint32(5)) & np.uint32(63)).astype(np.uint8)
+        k = self.plan_c & np.uint32(7)
+        t[(k != abi.CPLAN_PREVOTE) & (k != abi.CPLAN_VOTE)] = abi.CTAG_NONE
+        return t
 
 
 def outbox_in_block(block: np.ndarray, out_off, rows: int, n: int, F: int, esc_cap: int) -> CompactOutbox:
@@ -125,9 +139,9 @@ def inbox_in_block(block: np.ndarray, in_off, ci: CompactInbox) -> CompactInbox:
     return out
 
 
-def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray) -> tuple[CompactRequests, np.ndarray]:
+def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray, elections: bool = False) -> tuple[CompactRequests, np.ndarray]:
     """The request list of a dense inbox: every op other than a SUBMIT / TIMEOUT without a draw, in slot order.  Returns it
-    and the mask of the slots it carries (op_c leaves them NONE)."""
+    and the mask of the slots it carries (op_c leaves them NONE).  elections: PreVote / RequestVote become records too."""
     rows, n = ib.rows, ib.n
     draw = ib.op_nr["y"]
     listed = (ok != 0) & (((ok != abi.OP_SUBMIT) & (ok != abi.OP_TIMEOUT)) | (draw != 0))
@@ -153,11 +167,17 @@ def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray) -> tuple[C
             (dcommit >= -(1 << 31)) & (dcommit < (1 << 31)) & (dt >= 0) & (dt <= 0xFFFF) & (count <= 63) & (peer < 32) & in_pool)
     for k in np.flatnonzero(fits & (count > 0)):                               # every entry carries the request's term
         fits[k] = bool((ib.ent_terms[ent[k]:ent[k] + count[k]] == a[k]).all())
+    vk = np.zeros(len(at), np.int64)
+    if elections:                                                              # a record stands for d = e = 0, no entries
+        vk = np.where(kind == abi.OP_PREVOTE_REQ, abi.CREQ_VOTE_PRE, np.where(kind == abi.OP_VOTE_REQ, abi.CREQ_VOTE_RV, 0))
+        e_ok = (e == 0) if ib.op_e is not None else np.ones(len(at), bool)
+        fits |= ((vk != 0) & (dr == 0) & (count == 0) & (ent == 0) & (d == 0) & e_ok & (dterm < U64(1 << 32)) &
+                 (dt >= 0) & (dt <= 0xFFFF) & (peer < 32))
     req = np.zeros(int(fits.sum()), dtype=abi.CREQ)
     req["slot"] = at[fits]
-    req["meta"] = (peer[fits] | (count[fits] << 5) | (dt[fits] << 16)).astype(np.uint32)
+    req["meta"] = (peer[fits] | (count[fits] << 5) | (vk[fits] << 11) | (dt[fits] << 16)).astype(np.uint32)
     req["term"], req["prev_index"] = a[fits], b[fits]
-    req["d_prev_term"], req["d_commit"] = dterm[fits].astype(np.uint32), dcommit[fits].astype(np.int32)
+    req["d_prev_term"], req["d_commit"] = dterm[fits].astype(np.uint32), np.where(vk[fits] != 0, 0, dcommit[fits]).astype(np.int32)
     esc_k = np.flatnonzero(~fits)
     op_esc = np.zeros(len(esc_k), dtype=abi.CESC_OP)
     terms, pos = [], 0
@@ -170,7 +190,9 @@ def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray) -> tuple[C
     return CompactRequests(req, op_esc, np.concatenate(terms).astype(np.int64) if terms else None), listed
 
 
-def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray | None, sent_inc: np.ndarray | None = None) -> CompactInbox:
+def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray | None, sent_inc: np.ndarray | None = None,
+                 elections: bool = False, ballot_term: np.ndarray | None = None, ballot_inc: np.ndarray | None = None,
+                 ballot_tags: np.ndarray | None = None) -> CompactInbox:
     """ib: dense host inbox (any group ops, any lane events).
     tags[r, i, f]: the tag the RPC this event answers was sent under (plan_c of the step that emitted it); None = no acks yet.
     sent_term[i] / sent_inc[i]: the term those RPCs carried and the incarnation of the role object that sent them (the group's
@@ -178,7 +200,14 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     it with the echo pair under the tag — so a reply whose incarnation differs from sent_inc (a plan that was itself escaped)
     travels in full.
     Inbound requests, and SUBMIT / TIMEOUT ops with an explicit election-timeout draw, go to the request list `.reqs`
-    (CompactRequests; None when the step has none: then it is a RAFTING_INBOX_NO_REQUESTS step)."""
+    (CompactRequests; None when the step has none: then it is a RAFTING_INBOX_NO_REQUESTS step).
+    elections: the inbox of a step begun with abi.COMPACT_ELECTIONS.  Vote replies become ev_c words, PreVote / RequestVote
+    requests become records, and every escaped word carries the tag of the RPC it answers, which unpack frees: an ack's from
+    tags, which must then name AE / IS plans in flight only (CompactOutbox.tags(rpc_only=True)), a vote reply's from
+    ballot_tags[r, i, f] (CompactOutbox.ballot_tags() of the step that emitted the ballot; None = no compact ballot, every
+    vote reply travels in full).  ballot_term[r, i] / ballot_inc[r, i]: the term and the asking incarnation of the ballot the
+    vote replies in (r, i) answer (the decoded ballot columns of that step); a reply whose incarnation differs travels in
+    full."""
     rows, n, F = ib.rows, ib.n, ib.F
     if ib.gids is not None:
         raise ValueError("the compact path is dense (no active list)")
@@ -195,7 +224,7 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     c.row_base[:] = base
     c.reqs = None
     if has_op:
-        reqs, listed = _encode_requests(ib, ok, base)
+        reqs, listed = _encode_requests(ib, ok, base, elections)
         if listed.any():
             c.reqs = reqs
             ok = np.where(listed, U64(0), ok)
@@ -227,7 +256,25 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     fits = is_ack & (dt >= 0) & (dt <= 0xFFFF) & (tg < 32) & ((outcome != abi.OUT_OK) | term_ok) & inc_ok
     word = (em & U64(0x7F)) | (np.where(outcome == abi.OUT_OK, 1, 0).astype(np.uint64) << U64(7)) | (tg.astype(np.uint64) << U64(8)) | \
            (dt.astype(np.uint64) << U64(16))
-    c.ev_c[:] = np.where(fits, word, np.where(ek != 0, U64(abi.CEV_ESCAPED), U64(0))).astype(np.uint32)
+    escaped = U64(abi.CEV_ESCAPED)
+    if elections:
+        is_vote = (ek == abi.EV_PV_REPLY) | (ek == abi.EV_RV_REPLY)
+        bt = (ballot_term if ballot_term is not None else np.zeros((rows, n), np.int64))[:, :, None].astype(np.uint64)
+        binc = (ballot_inc if ballot_inc is not None else np.zeros((rows, n), np.uint64))[:, :, None].astype(np.uint64)
+        rt = ib.ev_tn["x"].astype(np.uint64)
+        is_ok = outcome == abi.OUT_OK
+        cterm = np.where(is_ok, bt - rt, U64(0))                                 # modulo 2^64: a higher term wraps past 7
+        # only a compact ballot lane's tag answers a vote: an AE / IS tag on the same lane belongs to a plan still in flight
+        tb = ballot_tags if ballot_tags is not None else np.full((rows, n, F), abi.CTAG_NONE, np.uint8)
+        vfits = (is_vote & (dt >= 0) & (dt <= 0xFFFF) & (tb < 32) & (np.where(is_ok, cterm < U64(8), rt == U64(0))) &
+                ((em >> U64(32)) == binc))
+        vword = (em & U64(0x7F)) | ((tb.astype(np.uint64) & U64(0x1F)) << U64(8)) | (np.where(vfits, cterm, U64(0)) << U64(13)) | \
+                (dt.astype(np.uint64) << U64(16))
+        word = np.where(is_vote, vword, word)
+        fits = fits | vfits
+        own = np.where(is_ack, tg, np.where(is_vote, tb, abi.CTAG_NONE)).astype(np.uint64)
+        escaped = U64(abi.CEV_ESCAPED) | (own << U64(8))                      # the escaped event's RPC frees its tag
+    c.ev_c[:] = np.where(fits, word, np.where(ek != 0, escaped, U64(0))).astype(np.uint32)
     esc_at = np.flatnonzero(((ek != 0) & ~fits).reshape(-1))
     if len(esc_at):
         c.esc = np.zeros(len(esc_at), dtype=abi.CESC_IN)
@@ -238,14 +285,25 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     return c
 
 
-def decode_outbox(co: CompactOutbox, G: int | None = None) -> abi.Outbox:
-    """The dense outbox a compact step stands for (rep_term / ballots / escaped plans come from the escape list)."""
+def decode_outbox(co: CompactOutbox, G: int | None = None, elections: bool = False) -> abi.Outbox:
+    """The dense outbox a compact step stands for (rep_term / ballots / escaped plans come from the escape list).
+    elections: the step was begun with abi.COMPACT_ELECTIONS, so plan_c lanes of kind CPLAN_PREVOTE / CPLAN_VOTE are ballots."""
     rows, n, F = co.rows, co.n, co.F
     if int(co.counts[0]) > co.esc_cap:
         raise OverflowError("escape list overflow: fetch the dense outbox (rafting_step_fetch_dense)")
     o = abi.Outbox(rows, n, F, n if G is None else G)
     pc = co.plan_c.astype(np.uint64)
     kind = (pc & U64(7)).astype(np.int64)
+    if elections and F:
+        bk = kind[:, :, 0]                                                       # every lane of a compact ballot has the word
+        pre, vote = bk == abi.CPLAN_PREVOTE, bk == abi.CPLAN_VOTE
+        has = pre | vote
+        o.ballot_meta[:] = np.where(has, np.where(pre, U64(abi.BALLOT_PREVOTE), U64(abi.BALLOT_VOTE)) |
+                                    (co.incarnation.astype(np.uint64)[None, :] << U64(32)), U64(0))
+        o.ballot_term[:] = np.where(has, co.current_term[None, :] + pre.astype(np.int64), 0)
+        o.ballot_last["x"] = np.where(has, co.last_entry["x"][None, :], 0)
+        o.ballot_last["y"] = np.where(has, co.last_entry["y"][None, :], 0)
+        kind = np.where(kind >= abi.CPLAN_PREVOTE, 0, kind)
     hb = (pc >> U64(3)) & U64(1)
     esc = ((pc >> U64(4)) & U64(1)) != 0
     cnt = ((pc >> U64(11)) & U64(63)).astype(np.int64)

@@ -8,6 +8,9 @@
 //                   every AE / IS plan gets a free tag of its (group, follower) lane and parks its echo pair and its
 //                   incarnation in the table; whatever breaks a compact rule goes, in full, to the escape list
 //
+// Under RAFTING_COMPACT_ELECTIONS (the EL instantiations) vote RPCs take tags as well: a compact ballot's lanes park
+// (ballot term, 0) and the asking role's incarnation, and a vote reply word gets them back.
+//
 // One thread per (group, follower) walks the rows in order in both kernels, so the tag bitmap of a lane is only ever touched
 // by its own thread, and the three kernels of a step (unpack, step, pack) are ordered on the engine's stream.  What this
 // replaces in the reference is the closure state of the Async callbacks registered by Leader.replicateLog
@@ -37,6 +40,8 @@ struct COutD {                                   // device view of rafting_coutb
     bool compact_replies;                        // rep_c bits 6 / 7 (steps begun with a request list)
 };
 
+// EL: steps begun with RAFTING_COMPACT_ELECTIONS (vote replies as words, escaped words that free their tag)
+template <bool EL>
 __global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW out, const i64x2* __restrict__ table, const uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits) {
     const uint32_t GF = T.G * T.F;
     const uint32_t t = blockIdx.x * 256u + threadIdx.x;
@@ -57,6 +62,21 @@ __global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW o
                 i64x2 tn; tn.x = ((w >> 7) & 1u) ? term_now : 0; tn.y = in.row_base[r] + (int64_t)(w >> 16);
                 em = (uint64_t)(w & 0x7fu) | ((uint64_t)inc << 32);         // kind | outcome | success | incarnation (from the table)
                 out.ev_tn[idx] = tn; out.ev_el[idx] = el;
+            } else if constexpr (EL) {
+                if (kind == RAFTING_EV_PV_REPLY || kind == RAFTING_EV_RV_REPLY) {
+                    // (ballot term, 0) and the asking role's incarnation wait under the tag; the reply's term is c below it
+                    const uint32_t tag = RAFTING_CEV_VOTE_TAG(w);
+                    const int64_t bt = table[(size_t)tag * GF + t].x; const uint32_t inc = tinc[(size_t)tag * GF + t];
+                    b &= ~(1u << tag);
+                    i64x2 tn; tn.x = ((w >> 4) & 3u) == RAFTING_OUT_OK ? (int64_t)((uint64_t)bt - RAFTING_CEV_VOTE_C(w)) : 0;
+                    tn.y = in.row_base[r] + (int64_t)(w >> 16);
+                    const i64x2 el = {0, 0};
+                    em = (uint64_t)(w & 0x7fu) | ((uint64_t)inc << 32);
+                    out.ev_tn[idx] = tn; out.ev_el[idx] = el;
+                } else if (kind == RAFTING_CEV_ESCAPED) {
+                    const uint32_t tag = (w >> 8) & 0xffu;                  // the escaped event's RPC has completed too
+                    if (tag < (uint32_t)CTAGS) b &= ~(1u << tag);
+                }
             }
             out.ev_meta[idx] = em;                                          // escaped / empty slots read as "no event" until patched
         }
@@ -85,6 +105,7 @@ struct CReqD {                                   // device view of rafting_creqs
     uint32_t* order;                             // bit 0: req decreases somewhere, bit 1: esc does
 };
 constexpr uint32_t CREQ_META_ZERO = 0xf800u;     // bits 11..15 of a record's meta
+constexpr uint32_t CREQ_META_ZERO_EL = 0xe000u;  // bits 13..15 (under RAFTING_COMPACT_ELECTIONS bits 11..12 name a vote)
 
 // Pass 1, one thread per list position: entry counts for the scan, and whether either list decreases anywhere.  A
 // decreasing list can hold the same slot twice at positions that are not adjacent; rather than search for them, every
@@ -116,6 +137,8 @@ __device__ __forceinline__ void put_op(const InboxW& o, size_t gi, uint64_t meta
 // Pass 2, one thread per record (k < n_req) or op escape (k - n_req): the op in full at its slot.  Every writer of a slot
 // that is claimed twice detects it from read-only inputs and writes the same malformed op, so the result never depends on
 // the order of the writes.
+// EL (RAFTING_COMPACT_ELECTIONS): a record with meta bits 11..12 set is a PreVote / RequestVote
+template <bool EL>
 __global__ void unpack_requests_kernel(CReqD q, InboxW o, uint32_t G) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if ((uint64_t)k >= (uint64_t)q.n_req + q.n_esc) return;
@@ -126,8 +149,21 @@ __global__ void unpack_requests_kernel(CReqD q, InboxW o, uint32_t G) {
     const uint32_t r = slot / G;
     bool bad = q.order[0] != 0 || (q.op_c && (q.op_c[slot] & 0xfu) != RAFTING_OP_NONE);
     if (is_req) {
-        bad = bad || (j > 0 && q.req[j - 1].slot == slot) || (j + 1 < q.n_req && q.req[j + 1].slot == slot) ||
-              list_holds(q.esc, q.n_esc, slot) || (q.req[j].meta & CREQ_META_ZERO) != 0;
+        if constexpr (EL) {
+            const uint32_t m = q.req[j].meta, vk = RAFTING_CREQ_VOTE(m);
+            bad = bad || (j > 0 && q.req[j - 1].slot == slot) || (j + 1 < q.n_req && q.req[j + 1].slot == slot) ||
+                  list_holds(q.esc, q.n_esc, slot) || (m & CREQ_META_ZERO_EL) != 0 || vk == 3u ||
+                  (vk != 0u && (RAFTING_CREQ_COUNT(m) != 0u || q.req[j].d_commit != 0));
+            if (!bad && vk != 0u) {
+                const rafting_creq_t x = q.req[j];
+                put_op(o, slot, (uint64_t)RAFTING_OP_MAKE(vk == RAFTING_CREQ_VOTE_PRE ? RAFTING_OP_PREVOTE_REQ : RAFTING_OP_VOTE_REQ, RAFTING_CREQ_PEER(m), 0u),
+                       q.row_base[r] + (int64_t)RAFTING_CREQ_DT(m), 0, x.term, x.prev_index, (int64_t)((uint64_t)x.term - (uint64_t)x.d_prev_term), 0, 0);
+                return;
+            }
+        } else {
+            bad = bad || (j > 0 && q.req[j - 1].slot == slot) || (j + 1 < q.n_req && q.req[j + 1].slot == slot) ||
+                  list_holds(q.esc, q.n_esc, slot) || (q.req[j].meta & CREQ_META_ZERO) != 0;
+        }
     } else {
         bad = bad || (j > 0 && q.esc[j - 1].slot == slot) || (j + 1 < q.n_esc && q.esc[j + 1].slot == slot) ||
               list_holds(q.req, q.n_req, slot);
@@ -169,6 +205,35 @@ __device__ __forceinline__ void put_escape(const COutD& o, uint32_t kind, uint32
     }
 }
 
+// Under RAFTING_COMPACT_ELECTIONS: the plan_c kind the ballot of (row, group) gi travels as, or 0 when it stays an escape
+// record.  Every lane thread of the group and its f == 0 thread reach the same answer from the same read-only columns.
+__device__ __forceinline__ uint32_t ballot_lane_kind(const OutboxD& in, size_t gi, uint32_t F, int64_t term_end, uint32_t inc_end, i64x2 last_end) {
+    if (!in.ballot_meta) return 0;
+    const uint64_t bm = in.ballot_meta[gi];
+    const uint32_t bk = (uint32_t)bm;                                   // bits 4..31 must be clear as well
+    if ((bk != RAFTING_BALLOT_PREVOTE && bk != RAFTING_BALLOT_VOTE) || (uint32_t)(bm >> 32) != inc_end) return 0;
+    const bool pre = bk == RAFTING_BALLOT_PREVOTE;
+    const i64x2 bl = in.ballot_last[gi];
+    if ((uint64_t)in.ballot_term[gi] != (uint64_t)term_end + (pre ? 1u : 0u) || bl.x != last_end.x || bl.y != last_end.y) return 0;
+    if (in.plan_meta)
+        for (uint32_t f = 0; f < F; f++) if (in.plan_meta[gi * F + f] != 0) return 0;
+    return pre ? RAFTING_CPLAN_PREVOTE : RAFTING_CPLAN_VOTE;
+}
+// the plan_c word of a compact ballot's lane: the lowest free tag of the lane parks (ballot term, 0) and the incarnation
+__device__ __forceinline__ uint32_t ballot_lane_word(const OutboxD& in, size_t gi, uint32_t F, int64_t term_end, uint32_t inc_end, i64x2 last_end,
+                                                     i64x2* table, uint32_t* tinc, size_t at, uint32_t& b) {
+    const uint32_t bk = ballot_lane_kind(in, gi, F, term_end, inc_end, last_end);
+    if (!bk) return 0;
+    uint32_t tag = RAFTING_CTAG_NONE;
+    const uint32_t fr = ~b;
+    if (fr) {
+        tag = (uint32_t)__ffs((int)fr) - 1u; b |= 1u << tag;
+        i64x2 v; v.x = in.ballot_term[gi]; v.y = 0; table[(size_t)tag * at] = v; tinc[(size_t)tag * at] = inc_end;
+    }
+    return bk | (tag << 5);
+}
+
+template <bool EL>
 __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, OutboxD in, COutD out, i64x2* __restrict__ table, uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits) {
     const uint32_t GF = T.G * T.F;
     const uint32_t t = blockIdx.x * 256u + threadIdx.x;
@@ -184,6 +249,9 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
             const size_t idx = (size_t)r * GF + t;
             const uint64_t pm = in.plan_meta[idx];
             uint32_t pc = 0;
+            if constexpr (EL) {
+                if (pm == 0) pc = ballot_lane_word(in, (size_t)r * T.G + g, T.F, term_end, inc_end, last_end, table + t, tinc + t, GF, b);
+            }
             if (pm != 0) {
                 const uint32_t kind = RAFTING_PLM_KIND(pm), count = RAFTING_PLM_COUNT(pm);
                 const i64x2 pp = in.plan_pp[idx], lc = in.plan_lc[idx];
@@ -211,6 +279,9 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
             }
             out.plan_c[idx] = pc;
         }
+    } else if constexpr (EL) {
+        for (uint32_t r = 0; r < rows; r++)
+            out.plan_c[(size_t)r * GF + t] = ballot_lane_word(in, (size_t)r * T.G + g, T.F, term_end, inc_end, last_end, table + t, tinc + t, GF, b);
     } else {
         for (uint32_t r = 0; r < rows; r++) out.plan_c[(size_t)r * GF + t] = 0;
     }
@@ -228,7 +299,16 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
             }
             out.rep_c[gi] = (uint8_t)rc;
             const uint64_t bm = in.ballot_meta ? in.ballot_meta[gi] : 0ull;
-            if (bm != 0) { atomicAdd(out.counts + 1, 1u); const i64x2 bl = in.ballot_last[gi]; put_escape(out, RAFTING_CESC_BALLOT, (uint32_t)gi, bm, in.ballot_term[gi], bl.x, bl.y, 0, 0); }
+            if constexpr (EL) {
+                if (bm != 0) {
+                    atomicAdd(out.counts + 1, 1u);
+                    if (!ballot_lane_kind(in, gi, T.F, term_end, inc_end, last_end)) {
+                        const i64x2 bl = in.ballot_last[gi]; put_escape(out, RAFTING_CESC_BALLOT, (uint32_t)gi, bm, in.ballot_term[gi], bl.x, bl.y, 0, 0);
+                    }
+                }
+            } else {
+                if (bm != 0) { atomicAdd(out.counts + 1, 1u); const i64x2 bl = in.ballot_last[gi]; put_escape(out, RAFTING_CESC_BALLOT, (uint32_t)gi, bm, in.ballot_term[gi], bl.x, bl.y, 0, 0); }
+            }
         }
         out.commit_index[g] = commit_end; out.current_term[g] = term_end; out.role_word[g] = in.role_word[g];
         out.incarnation[g] = inc_end; out.err_word[g] = in.err_word[g]; out.last_entry[g] = last_end; out.epoch[g] = epoch_end;
@@ -312,8 +392,15 @@ extern "C" int rafting_step_begin_compact(rafting_engine_t* e, uint32_t slot, co
 
 extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
                                               const rafting_coutbox_t* out) {
+    return rafting_step_begin_compact_ex(e, slot, in, reqs, out, 0u);
+}
+
+extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
+                                             const rafting_coutbox_t* out, uint32_t flags) {
     using namespace rafting;
     if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
+    if (flags & ~RAFTING_COMPACT_ELECTIONS) return fail(RAFTING_E_INVAL, "unknown compact step flags 0x%x", flags);
+    const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0;
     const bool has_reqs = reqs && (reqs->n_req || reqs->n_op_esc);
     if (!in->row_base || (!in->op_c && !in->ev_c && !has_reqs))
         return fail(RAFTING_E_INVAL, "compact inbox needs row_base and at least one of op_c / ev_c / a request");
@@ -425,7 +512,8 @@ extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot
     dw.op_meta = (uint64_t*)di.op_meta; dw.op_nr = (i64x2*)di.op_nr; dw.op_ab = (i64x2*)di.op_ab;
     dw.ev_meta = (uint64_t*)di.ev_meta; dw.ev_tn = (i64x2*)di.ev_tn; dw.ev_el = (i64x2*)di.ev_el;
     dw.op_cd = (i64x2*)di.op_cd; dw.op_e = (int64_t*)di.op_e; dw.ent_terms = (int64_t*)di.ent_terms;
-    unpack_kernel<<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits);
+    if (el) unpack_kernel<true><<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits);
+    else unpack_kernel<false><<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits);
     if (in->ev_c == nullptr && in->n_esc) CU(cudaMemsetAsync((void*)di.ev_meta, 0, rows * G * F * 8, e->stream));
     if (in->n_esc) unpack_escapes_kernel<<<(in->n_esc + 255u) / 256u, 256, 0, e->stream>>>(ci, dw, (uint32_t)(rows * G * F));
     if (has_reqs) {
@@ -439,12 +527,15 @@ extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot
         CU(cudaMemsetAsync(q.order, 0, 4, e->stream));
         creq_prepare_kernel<<<(most + 255u) / 256u, 256, 0, e->stream>>>(q);
         if (n_req) { size_t tb = scan_tmp; CU(cub::DeviceScan::ExclusiveSum(S.creqw.p + w_tmp, tb, q.counts, q.offs, (int)n_req, e->stream)); }
-        unpack_requests_kernel<<<(uint32_t)((n_req + n_oesc + 255u) / 256u), 256, 0, e->stream>>>(q, dw, (uint32_t)G);
+        const uint32_t rq_blocks = (uint32_t)((n_req + n_oesc + 255u) / 256u);
+        if (el) unpack_requests_kernel<true><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)G);
+        else unpack_requests_kernel<false><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)G);
     }
     CU(cudaGetLastError());
     rc = launch_step(e, di, dov, e->stream);
     if (rc) { cudaStreamSynchronize(H->s_h2d); return rc; }
-    pack_kernel<<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits);
+    if (el) pack_kernel<true><<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits);
+    else pack_kernel<false><<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits);
     CU(cudaGetLastError());
     CU(cudaEventRecord(S.ev_kernel, e->stream));
     // ---- D2H: every wire column + the counters; the escape list only when the counters say it holds something ----

@@ -428,7 +428,14 @@ template <typename Rec> void insert_at(Rec* v, uint32_t* n, uint32_t at, const R
 extern "C" int rafting_request_to_creq(const rafting_req_rec_t* r, const int64_t* entry_terms, uint32_t row, int64_t now_ms,
                                        int host_result, const rafting_cinbox_t* in, uint32_t n_groups, rafting_creqs_t* q,
                                        uint32_t req_cap, uint32_t esc_cap, uint32_t ent_cap) {
+    return rafting_request_to_creq_ex(r, entry_terms, row, now_ms, host_result, in, n_groups, q, req_cap, esc_cap, ent_cap, 0u);
+}
+
+extern "C" int rafting_request_to_creq_ex(const rafting_req_rec_t* r, const int64_t* entry_terms, uint32_t row, int64_t now_ms,
+                                          int host_result, const rafting_cinbox_t* in, uint32_t n_groups, rafting_creqs_t* q,
+                                          uint32_t req_cap, uint32_t esc_cap, uint32_t ent_cap, uint32_t flags) {
     if (!r || !in || !in->row_base || !q || (q->n_req && !q->req) || (q->n_op_esc && !q->op_esc)) return RAFTING_E_INVAL;
+    if (flags & ~RAFTING_COMPACT_ELECTIONS) return RAFTING_E_INVAL;
     if (r->gid >= n_groups || row >= in->rows) return RAFTING_E_INVAL;
     if (r->kind != RAFTING_OP_AE_REQUEST && r->kind != RAFTING_OP_PREVOTE_REQ && r->kind != RAFTING_OP_VOTE_REQ &&
         r->kind != RAFTING_OP_IS_REQUEST) return RAFTING_E_INVAL;
@@ -447,6 +454,16 @@ extern "C" int rafting_request_to_creq(const rafting_req_rec_t* r, const int64_t
     bool fits = ae && count <= 63 && r->src_slot < 32 && dt >= 0 && dt <= 0xFFFF && dterm < (1ull << 32) &&
                 dcommit >= INT32_MIN && dcommit <= INT32_MAX;
     for (uint32_t i = 0; fits && i < count; i++) fits = entry_terms[i] == r->term;
+    const bool vote = r->kind == RAFTING_OP_PREVOTE_REQ || r->kind == RAFTING_OP_VOTE_REQ;
+    if ((flags & RAFTING_COMPACT_ELECTIONS) && vote && r->src_slot < 32 && dt >= 0 && dt <= 0xFFFF && dterm < (1ull << 32)) {
+        if (q->n_req >= req_cap) return RAFTING_E_INVAL;                  // a vote record: (lastLogIndex, term - lastLogTerm)
+        rafting_creq_t x;
+        x.slot = slot; x.term = r->term; x.prev_index = r->a; x.d_prev_term = (uint32_t)dterm; x.d_commit = 0;
+        x.meta = RAFTING_CREQ_MAKE(r->src_slot, 0u, (uint32_t)dt) |
+                 ((r->kind == RAFTING_OP_PREVOTE_REQ ? RAFTING_CREQ_VOTE_PRE : RAFTING_CREQ_VOTE_RV) << 11);
+        insert_at(req, &q->n_req, at_req, x);
+        return RAFTING_OK;
+    }
     if (fits) {
         if (q->n_req >= req_cap) return RAFTING_E_INVAL;
         rafting_creq_t x;
@@ -606,8 +623,17 @@ extern "C" int rafting_pending_remove(rafting_pending_t* p, uint32_t peer, int32
 extern "C" int rafting_acks_to_cinbox(rafting_pending_t* p, uint32_t peer, const rafting_ack_rec_t* acks, uint32_t n, int64_t now_ms,
                                       uint32_t row, const rafting_cinbox_t* cin, uint32_t n_groups, uint32_t F, rafting_cesc_in_t* esc,
                                       uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred, uint32_t* n_deferred, uint32_t* n_unknown) {
-    if (!p || (!acks && n) || !cin || !cin->ev_c || !cin->row_base || !n_esc || !n_deferred || (!deferred && n) || row >= cin->rows)
+    return rafting_acks_to_cinbox_ex(p, peer, acks, n, now_ms, row, cin, n_groups, F, esc, esc_cap, n_esc, deferred, n_deferred, n_unknown, 0u);
+}
+
+extern "C" int rafting_acks_to_cinbox_ex(rafting_pending_t* p, uint32_t peer, const rafting_ack_rec_t* acks, uint32_t n, int64_t now_ms,
+                                         uint32_t row, const rafting_cinbox_t* cin, uint32_t n_groups, uint32_t F, rafting_cesc_in_t* esc,
+                                         uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred, uint32_t* n_deferred, uint32_t* n_unknown,
+                                         uint32_t flags) {
+    if (!p || (!acks && n) || !cin || !cin->ev_c || !cin->row_base || !n_esc || !n_deferred || (!deferred && n) || row >= cin->rows ||
+        (flags & ~RAFTING_COMPACT_ELECTIONS))
         return RAFTING_E_INVAL;
+    const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0;
     uint32_t* ev = const_cast<uint32_t*>(cin->ev_c);
     const int64_t dt = now_ms - cin->row_base[row];
     uint32_t unknown = 0, nd = 0;
@@ -623,9 +649,13 @@ extern "C" int rafting_acks_to_cinbox(rafting_pending_t* p, uint32_t peer, const
         const size_t li = ((size_t)row * n_groups + e->gid) * F + e->lane;
         if (ev[li] != 0) { deferred[nd++] = i; continue; }                    // one event per (row, group, lane)
         const bool is_ack = a.kind == RAFTING_EV_AE_ACK || a.kind == RAFTING_EV_IS_ACK;
+        const bool is_vote = el && (a.kind == RAFTING_EV_PV_REPLY || a.kind == RAFTING_EV_RV_REPLY);
+        const uint64_t c = (uint64_t)e->term - (uint64_t)a.term;              // votes: ballot term - RaftResponse.term()
         const bool fits = is_ack && e->tag < 32 && dt >= 0 && dt <= 0xFFFF && a.term == e->term;
         if (fits) {
             ev[li] = RAFTING_CEV_MAKE(a.kind, RAFTING_OUT_OK, a.success ? 1 : 0, 1, e->tag, (uint32_t)dt);
+        } else if (is_vote && e->tag < 32 && dt >= 0 && dt <= 0xFFFF && c < 8u) {
+            ev[li] = RAFTING_CEV_VOTE_MAKE(a.kind, RAFTING_OUT_OK, a.success ? 1 : 0, e->tag, (uint32_t)c, (uint32_t)dt);
         } else {
             if (!esc || *n_esc >= esc_cap) { *n_deferred = nd; if (n_unknown) *n_unknown = unknown; return RAFTING_E_CAPACITY; }
             rafting_cesc_in_t& x = esc[(*n_esc)++];
@@ -633,7 +663,7 @@ extern "C" int rafting_acks_to_cinbox(rafting_pending_t* p, uint32_t peer, const
             x.slot = (uint32_t)li;
             x.ev_meta = RAFTING_EVM_MAKE(a.kind, RAFTING_OUT_OK, a.success ? 1 : 0, e->inc);
             x.term = a.term; x.now_ms = now_ms; x.epoch_at_send = e->epoch; x.last_at_send = e->last;
-            ev[li] = RAFTING_CEV_ESCAPED;
+            ev[li] = el ? RAFTING_CEV_ESCAPED | ((uint32_t)e->tag << 8) : RAFTING_CEV_ESCAPED;   // flagged: the escape frees the tag
         }
         p->erase(e);
     }
@@ -646,8 +676,17 @@ extern "C" int rafting_failures_to_cinbox(rafting_pending_t* p, uint32_t peer, c
                                           int64_t now_ms, uint32_t row, const rafting_cinbox_t* cin, uint32_t n_groups, uint32_t F,
                                           rafting_cesc_in_t* esc, uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred,
                                           uint32_t* n_deferred, uint32_t* n_unknown) {
+    return rafting_failures_to_cinbox_ex(p, peer, sequences, n, outcome, now_ms, row, cin, n_groups, F, esc, esc_cap, n_esc, deferred,
+                                         n_deferred, n_unknown, 0u);
+}
+
+extern "C" int rafting_failures_to_cinbox_ex(rafting_pending_t* p, uint32_t peer, const int32_t* sequences, uint32_t n, uint32_t outcome,
+                                             int64_t now_ms, uint32_t row, const rafting_cinbox_t* cin, uint32_t n_groups, uint32_t F,
+                                             rafting_cesc_in_t* esc, uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred,
+                                             uint32_t* n_deferred, uint32_t* n_unknown, uint32_t flags) {
     if (!p || (!sequences && n) || !cin || !cin->ev_c || !cin->row_base || !n_esc || !n_deferred || (!deferred && n) || row >= cin->rows ||
-        (outcome != RAFTING_OUT_ERROR && outcome != RAFTING_OUT_CANCELED)) return RAFTING_E_INVAL;
+        (outcome != RAFTING_OUT_ERROR && outcome != RAFTING_OUT_CANCELED) || (flags & ~RAFTING_COMPACT_ELECTIONS)) return RAFTING_E_INVAL;
+    const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0;
     uint32_t* ev = const_cast<uint32_t*>(cin->ev_c);
     const int64_t dt = now_ms - cin->row_base[row];
     uint32_t unknown = 0, nd = 0;
@@ -658,8 +697,11 @@ extern "C" int rafting_failures_to_cinbox(rafting_pending_t* p, uint32_t peer, c
         const size_t li = ((size_t)row * n_groups + e->gid) * F + e->lane;
         if (ev[li] != 0) { deferred[nd++] = i; continue; }
         const bool is_ack = e->kind == RAFTING_EV_AE_ACK || e->kind == RAFTING_EV_IS_ACK;
+        const bool is_vote = el && (e->kind == RAFTING_EV_PV_REPLY || e->kind == RAFTING_EV_RV_REPLY);
         if (is_ack && e->tag < 32 && dt >= 0 && dt <= 0xFFFF) {
             ev[li] = RAFTING_CEV_MAKE(e->kind, outcome, 0, 0, e->tag, (uint32_t)dt);
+        } else if (is_vote && e->tag < 32 && dt >= 0 && dt <= 0xFFFF) {
+            ev[li] = RAFTING_CEV_VOTE_MAKE(e->kind, outcome, 0, e->tag, 0u, (uint32_t)dt);
         } else {
             if (!esc || *n_esc >= esc_cap) { *n_deferred = nd; if (n_unknown) *n_unknown = unknown; return RAFTING_E_CAPACITY; }
             rafting_cesc_in_t& x = esc[(*n_esc)++];
@@ -667,7 +709,7 @@ extern "C" int rafting_failures_to_cinbox(rafting_pending_t* p, uint32_t peer, c
             x.slot = (uint32_t)li;
             x.ev_meta = RAFTING_EVM_MAKE(e->kind, outcome, 0, e->inc);
             x.term = 0; x.now_ms = now_ms; x.epoch_at_send = e->epoch; x.last_at_send = e->last;
-            ev[li] = RAFTING_CEV_ESCAPED;
+            ev[li] = el ? RAFTING_CEV_ESCAPED | ((uint32_t)e->tag << 8) : RAFTING_CEV_ESCAPED;
         }
         p->erase(e);
     }

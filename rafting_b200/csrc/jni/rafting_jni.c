@@ -116,6 +116,11 @@ JNIEXPORT void JNICALL FN(stepBeginCompactReq)(JNIEnv* env, jclass k, jlong h, j
     CHECK(rafting_step_begin_compact_req(ENG(h), (uint32_t)slot, (const rafting_cinbox_t*)BUF(cin), (const rafting_creqs_t*)BUF(creqs),
                                          (const rafting_coutbox_t*)BUF(cout)));
 }
+/* the same with RAFTING_COMPACT_ELECTIONS (or 0) in flags: ballots, vote replies and vote requests travel compact */
+JNIEXPORT void JNICALL FN(stepBeginCompactEx)(JNIEnv* env, jclass k, jlong h, jint slot, jobject cin, jobject creqs, jobject cout, jint flags) {
+    CHECK(rafting_step_begin_compact_ex(ENG(h), (uint32_t)slot, (const rafting_cinbox_t*)BUF(cin), (const rafting_creqs_t*)BUF(creqs),
+                                        (const rafting_coutbox_t*)BUF(cout), (uint32_t)flags));
+}
 JNIEXPORT void JNICALL FN(stepWaitCompact)(JNIEnv* env, jclass k, jlong h, jint slot) { CHECK(rafting_step_wait_compact(ENG(h), (uint32_t)slot)); }
 JNIEXPORT void JNICALL FN(stepFetchDense)(JNIEnv* env, jclass k, jlong h, jint slot, jobject outStruct) {
     CHECK(rafting_step_fetch_dense(ENG(h), (uint32_t)slot, (const rafting_outbox_t*)BUF(outStruct)));
@@ -274,6 +279,12 @@ JNIEXPORT void JNICALL FN(requestToCreq)(JNIEnv* env, jclass k, jobject rec, job
                                   (const rafting_cinbox_t*)BUF(cinStruct), (uint32_t)nGroups, (rafting_creqs_t*)BUF(creqsStruct),
                                   (uint32_t)reqCap, (uint32_t)escCap, (uint32_t)entCap));
 }
+JNIEXPORT void JNICALL FN(requestToCreqEx)(JNIEnv* env, jclass k, jobject rec, jobject entryTerms, jint row, jlong nowMs, jboolean hostResult,
+                                           jobject cinStruct, jint nGroups, jobject creqsStruct, jint reqCap, jint escCap, jint entCap, jint flags) {
+    CHECK(rafting_request_to_creq_ex((const rafting_req_rec_t*)BUF(rec), (const int64_t*)BUF(entryTerms), (uint32_t)row, nowMs, hostResult ? 1 : 0,
+                                     (const rafting_cinbox_t*)BUF(cinStruct), (uint32_t)nGroups, (rafting_creqs_t*)BUF(creqsStruct),
+                                     (uint32_t)reqCap, (uint32_t)escCap, (uint32_t)entCap, (uint32_t)flags));
+}
 JNIEXPORT jint JNICALL FN(coutboxToReplies)(JNIEnv* env, jclass k, jobject coutStruct, jint nGroups, jint localSlot, jobject placed,
                                             jobject placedRow, jint n, jobject repliesOut) {
     uint32_t got = 0;
@@ -315,6 +326,18 @@ JNIEXPORT void JNICALL FN(failuresToCinbox)(JNIEnv* env, jclass k, jlong p, jint
     if (c) { c[0] = nEsc; c[1] = nDef; c[2] = nUnknown; }
     if (rc) throw_status(env, rc);
 }
+JNIEXPORT void JNICALL FN(failuresToCinboxEx)(JNIEnv* env, jclass k, jlong p, jint peer, jobject sequences, jint n, jint outcome, jlong nowMs,
+                                              jint row, jobject cinStruct, jint nGroups, jint followers, jobject esc, jint escCap,
+                                              jobject deferredOut, jobject counters, jint flags) {
+    int64_t* c = (int64_t*)BUF(counters);
+    uint32_t nEsc = c ? (uint32_t)c[0] : 0, nDef = 0, nUnknown = 0;
+    int rc = rafting_failures_to_cinbox_ex((rafting_pending_t*)(intptr_t)p, (uint32_t)peer, (const int32_t*)BUF(sequences), (uint32_t)n,
+                                           (uint32_t)outcome, nowMs, (uint32_t)row, (const rafting_cinbox_t*)BUF(cinStruct), (uint32_t)nGroups,
+                                           (uint32_t)followers, (rafting_cesc_in_t*)BUF(esc), (uint32_t)escCap, &nEsc, (uint32_t*)BUF(deferredOut),
+                                           &nDef, &nUnknown, (uint32_t)flags);
+    if (c) { c[0] = nEsc; c[1] = nDef; c[2] = nUnknown; }
+    if (rc) throw_status(env, rc);
+}
 JNIEXPORT jboolean JNICALL FN(pendingRemove)(JNIEnv* env, jclass k, jlong p, jint peer, jint sequence) {
     return rafting_pending_remove((rafting_pending_t*)(intptr_t)p, (uint32_t)peer, sequence) == RAFTING_OK;
 }
@@ -326,6 +349,17 @@ JNIEXPORT void JNICALL FN(acksToCinbox)(JNIEnv* env, jclass k, jlong p, jint pee
     int rc = rafting_acks_to_cinbox((rafting_pending_t*)(intptr_t)p, (uint32_t)peer, (const rafting_ack_rec_t*)BUF(acks), (uint32_t)n, nowMs,
                                     (uint32_t)row, (const rafting_cinbox_t*)BUF(cinStruct), (uint32_t)nGroups, (uint32_t)followers,
                                     (rafting_cesc_in_t*)BUF(esc), (uint32_t)escCap, &nEsc, (uint32_t*)BUF(deferredOut), &nDef, &nUnknown);
+    if (c) { c[0] = nEsc; c[1] = nDef; c[2] = nUnknown; }
+    if (rc) throw_status(env, rc);
+}
+JNIEXPORT void JNICALL FN(acksToCinboxEx)(JNIEnv* env, jclass k, jlong p, jint peer, jobject acks, jint n, jlong nowMs, jint row, jobject cinStruct,
+                                          jint nGroups, jint followers, jobject esc, jint escCap, jobject deferredOut, jobject counters, jint flags) {
+    int64_t* c = (int64_t*)BUF(counters);
+    uint32_t nEsc = c ? (uint32_t)c[0] : 0, nDef = 0, nUnknown = 0;
+    int rc = rafting_acks_to_cinbox_ex((rafting_pending_t*)(intptr_t)p, (uint32_t)peer, (const rafting_ack_rec_t*)BUF(acks), (uint32_t)n, nowMs,
+                                       (uint32_t)row, (const rafting_cinbox_t*)BUF(cinStruct), (uint32_t)nGroups, (uint32_t)followers,
+                                       (rafting_cesc_in_t*)BUF(esc), (uint32_t)escCap, &nEsc, (uint32_t*)BUF(deferredOut), &nDef, &nUnknown,
+                                       (uint32_t)flags);
     if (c) { c[0] = nEsc; c[1] = nDef; c[2] = nUnknown; }
     if (rc) throw_status(env, rc);
 }

@@ -38,7 +38,7 @@ EXPORTS = [
     "rafting_comm_init", "rafting_comm_init_all", "rafting_comm_unique_id", "rafting_allgather_commit", "rafting_allgather_commit_from",
     "rafting_allgather_commit_all", "rafting_allgather_last", "rafting_restore_async", "rafting_state_save", "rafting_state_load", "rafting_step_device_seq", "rafting_engine_stream",
     "rafting_engine_counters", "rafting_abi_sizes", "rafting_checkpoint", "rafting_restore",
-    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
+    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
     "rafting_log_config", "rafting_log_append", "rafting_log_read", "rafting_log_gather", "rafting_log_trim", "rafting_log_stats",
     "rafting_log_store_open", "rafting_log_sync", "rafting_log_mark", "rafting_log_recovered", "rafting_log_export_kv", "rafting_log_store_stats",
 ]
@@ -115,6 +115,8 @@ def lib():
         L.rafting_step_begin_compact.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.CInboxC), C.POINTER(abi.COutboxC)]
         L.rafting_step_begin_compact_req.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.CInboxC), C.POINTER(abi.CReqsC),
                                                      C.POINTER(abi.COutboxC)]
+        L.rafting_step_begin_compact_ex.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.CInboxC), C.POINTER(abi.CReqsC),
+                                                    C.POINTER(abi.COutboxC), C.c_uint32]
         L.rafting_compact_req_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 4)]
         L.rafting_step_wait_compact.argtypes = [C.c_void_p, C.c_uint32]
         L.rafting_compact_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 6),
@@ -240,10 +242,17 @@ class Engine:
         _check(lib().rafting_compact_req_layout(n_req, n_op_esc, ent_count, C.byref(a)), "rafting_compact_req_layout")
         return list(a)
 
-    def step_compact(self, cin, cout, slot: int = 0, reqs=None):
+    def step_begin_compact_ex(self, slot: int, cin_c: abi.CInboxC, reqs_c: abi.CReqsC | None, cout_c: abi.COutboxC, flags: int):
+        _check(lib().rafting_step_begin_compact_ex(self._h, slot, C.byref(cin_c), None if reqs_c is None else C.byref(reqs_c),
+                                                   C.byref(cout_c), flags), "rafting_step_begin_compact_ex")
+
+    def step_compact(self, cin, cout, slot: int = 0, reqs=None, flags: int = 0):
         """Synchronous compact step: cin / cout are rafting_b200.compact.CompactInbox / CompactOutbox, reqs a
-        rafting_b200.compact.CompactRequests (None: rafting_step_begin_compact)."""
-        if reqs is None:
+        rafting_b200.compact.CompactRequests (None: rafting_step_begin_compact).  flags = abi.COMPACT_ELECTIONS carries
+        ballots, vote replies and vote requests compact (rafting_step_begin_compact_ex)."""
+        if flags:
+            self.step_begin_compact_ex(slot, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags)
+        elif reqs is None:
             self.step_begin_compact(slot, cin.as_c(), cout.as_c())
         else:
             self.step_begin_compact_req(slot, cin.as_c(), reqs.as_c(), cout.as_c())

@@ -57,6 +57,7 @@ def lib():
                                                 C.c_void_p, C.POINTER(C.c_uint32)]
         L.rafting_request_to_creq.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int64, C.c_int, C.POINTER(abi.CInboxC),
                                               C.c_uint32, C.POINTER(abi.CReqsC), C.c_uint32, C.c_uint32, C.c_uint32]
+        L.rafting_request_to_creq_ex.argtypes = L.rafting_request_to_creq.argtypes + [C.c_uint32]
         L.rafting_coutbox_to_replies.argtypes = [C.POINTER(abi.COutboxC), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
                                                  C.c_void_p, C.POINTER(C.c_uint32)]
         L.rafting_outbox_apply_ranges.argtypes = [C.POINTER(abi.OutboxC), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
@@ -68,12 +69,14 @@ def lib():
         L.rafting_failures_to_cinbox.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32,
                                                  C.POINTER(abi.CInboxC), C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32),
                                                  C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+        L.rafting_failures_to_cinbox_ex.argtypes = L.rafting_failures_to_cinbox.argtypes + [C.c_uint32]
         L.rafting_pending_remove.argtypes = [C.c_void_p, C.c_uint32, C.c_int32]
         L.rafting_pending_size.restype = C.c_uint32
         L.rafting_pending_size.argtypes = [C.c_void_p]
         L.rafting_acks_to_cinbox.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint32, C.POINTER(abi.CInboxC),
                                              C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_void_p,
                                              C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+        L.rafting_acks_to_cinbox_ex.argtypes = L.rafting_acks_to_cinbox.argtypes + [C.c_uint32]
         L.rafting_builder_create.argtypes = [C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
         L.rafting_builder_destroy.argtypes = [C.c_void_p]
         L.rafting_builder_push_submit.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
@@ -248,13 +251,15 @@ class CReqPlacer:
         self.c = abi.CReqsC()
         self.c.req, self.c.op_esc, self.c.ent_terms = self.req.ctypes.data, self.op_esc.ctypes.data, self.ent_terms.ctypes.data
 
-    def put(self, rec, entry_terms, row: int, now_ms: int, host_result: bool, cin, n_groups: int) -> int:
-        """One request record -> a record or an op escape at (row, rec.gid) of the compact step `cin`; returns the status code."""
+    def put(self, rec, entry_terms, row: int, now_ms: int, host_result: bool, cin, n_groups: int, flags: int = 0) -> int:
+        """One request record -> a record or an op escape at (row, rec.gid) of the compact step `cin`; returns the status code.
+        flags = abi.COMPACT_ELECTIONS: PreVote / RequestVote become vote records (rafting_request_to_creq_ex)."""
         r = np.array([rec], dtype=REQ_REC)
         terms = np.ascontiguousarray(entry_terms, dtype=np.int64)
         ic = cin.as_c()
-        return lib().rafting_request_to_creq(r.ctypes.data, terms.ctypes.data if len(terms) else None, row, now_ms, 1 if host_result else 0,
-                                             C.byref(ic), n_groups, C.byref(self.c), *self.caps)
+        args = (r.ctypes.data, terms.ctypes.data if len(terms) else None, row, now_ms, 1 if host_result else 0, C.byref(ic), n_groups,
+                C.byref(self.c), *self.caps)
+        return lib().rafting_request_to_creq_ex(*args, flags) if flags else lib().rafting_request_to_creq(*args)
 
     def requests(self):
         """-> rafting_b200.compact.CompactRequests (copies of the lists placed so far)"""
@@ -312,25 +317,29 @@ class Pending:
     def __len__(self):
         return lib().rafting_pending_size(self._h)
 
-    def acks_to_cinbox(self, peer: int, acks: np.ndarray, now_ms: int, row: int, cin, esc: np.ndarray, n_esc: int):
+    def acks_to_cinbox(self, peer: int, acks: np.ndarray, now_ms: int, row: int, cin, esc: np.ndarray, n_esc: int, flags: int = 0):
         """Writes the replies into row `row` of the compact inbox `cin` (rafting_b200.compact.CompactInbox with ev_c allocated);
-        -> (status, escape records used so far, indices of deferred acks, unknown sequences)."""
+        -> (status, escape records used so far, indices of deferred acks, unknown sequences).  flags = abi.COMPACT_ELECTIONS:
+        vote replies become vote words and escaped words carry their tag (rafting_acks_to_cinbox_ex)."""
         acks = np.ascontiguousarray(acks, dtype=ACK_REC)
         deferred = np.zeros(max(1, len(acks)), dtype=np.uint32)
         ne, nd, nu = C.c_uint32(n_esc), C.c_uint32(), C.c_uint32()
         cc = cin.as_c()
-        rc = lib().rafting_acks_to_cinbox(self._h, peer, acks.ctypes.data, len(acks), now_ms, row, C.byref(cc), cin.n, cin.F,
-                                          esc.ctypes.data, len(esc), C.byref(ne), deferred.ctypes.data, C.byref(nd), C.byref(nu))
+        args = (self._h, peer, acks.ctypes.data, len(acks), now_ms, row, C.byref(cc), cin.n, cin.F, esc.ctypes.data, len(esc), C.byref(ne),
+                deferred.ctypes.data, C.byref(nd), C.byref(nu))
+        rc = lib().rafting_acks_to_cinbox_ex(*args, flags) if flags else lib().rafting_acks_to_cinbox(*args)
         return rc, ne.value, deferred[:nd.value].copy(), nu.value
 
-    def failures_to_cinbox(self, peer: int, sequences, outcome: int, now_ms: int, row: int, cin, esc: np.ndarray, n_esc: int):
+    def failures_to_cinbox(self, peer: int, sequences, outcome: int, now_ms: int, row: int, cin, esc: np.ndarray, n_esc: int,
+                           flags: int = 0):
         """Invocations that timed out (OUT_ERROR) / were cancelled (OUT_CANCELED): same contract as acks_to_cinbox."""
         seqs = np.ascontiguousarray(sequences, dtype=np.int32)
         deferred = np.zeros(max(1, len(seqs)), dtype=np.uint32)
         ne, nd, nu = C.c_uint32(n_esc), C.c_uint32(), C.c_uint32()
         cc = cin.as_c()
-        rc = lib().rafting_failures_to_cinbox(self._h, peer, seqs.ctypes.data, len(seqs), outcome, now_ms, row, C.byref(cc), cin.n, cin.F,
-                                              esc.ctypes.data, len(esc), C.byref(ne), deferred.ctypes.data, C.byref(nd), C.byref(nu))
+        args = (self._h, peer, seqs.ctypes.data, len(seqs), outcome, now_ms, row, C.byref(cc), cin.n, cin.F, esc.ctypes.data, len(esc),
+                C.byref(ne), deferred.ctypes.data, C.byref(nd), C.byref(nu))
+        rc = lib().rafting_failures_to_cinbox_ex(*args, flags) if flags else lib().rafting_failures_to_cinbox(*args)
         return rc, ne.value, deferred[:nd.value].copy(), nu.value
 
     def __del__(self):

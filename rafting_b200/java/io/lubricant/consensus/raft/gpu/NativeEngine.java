@@ -30,6 +30,7 @@ final class NativeEngine {
     static native void stepWaitSlot(long h, int slot);                                           // rafting_step_wait_slot
     static native void stepBeginCompact(long h, int slot, ByteBuffer cinbox, ByteBuffer coutbox); // rafting_step_begin_compact (§7)
     static native void stepBeginCompactReq(long h, int slot, ByteBuffer cinbox, ByteBuffer creqs, ByteBuffer coutbox);   // rafting_step_begin_compact_req: with inbound requests
+    static native void stepBeginCompactEx(long h, int slot, ByteBuffer cinbox, ByteBuffer creqs, ByteBuffer coutbox, int flags);   // rafting_step_begin_compact_ex: RAFTING_COMPACT_ELECTIONS
     static native void stepWaitCompact(long h, int slot);                                        // rafting_step_wait_compact
     static native void stepFetchDense(long h, int slot, ByteBuffer outboxStruct);                // rafting_step_fetch_dense (escape overflow)
     static native void checkpoint(long h);                                                       // rafting_checkpoint
@@ -63,9 +64,13 @@ final class NativeEngine {
     static native void pendingPut(long p, int peer, int sequence, int evKind, int gid, int lane, int tag, int incarnation, long term, long epochAtSend, long lastAtSend);
     static native void failuresToCinbox(long p, int peer, ByteBuffer sequences, int n, int outcome, long nowMs, int row, ByteBuffer cinStruct, int nGroups, int followers,
                                         ByteBuffer esc, int escCap, ByteBuffer deferredOut, ByteBuffer counters);   // Async time-outs / cancellations -> ev_c words
+    static native void failuresToCinboxEx(long p, int peer, ByteBuffer sequences, int n, int outcome, long nowMs, int row, ByteBuffer cinStruct, int nGroups,
+                                          int followers, ByteBuffer esc, int escCap, ByteBuffer deferredOut, ByteBuffer counters, int flags);   // the same for a flagged step
     static native boolean pendingRemove(long p, int peer, int sequence);                         // the invocation timed out
     static native void acksToCinbox(long p, int peer, ByteBuffer ackRecs, int n, long nowMs, int row, ByteBuffer cinStruct, int nGroups, int followers,
                                     ByteBuffer esc, int escCap, ByteBuffer deferredOut, ByteBuffer counters);   // replies -> ev_c words / escape records
+    static native void acksToCinboxEx(long p, int peer, ByteBuffer ackRecs, int n, long nowMs, int row, ByteBuffer cinStruct, int nGroups, int followers,
+                                      ByteBuffer esc, int escCap, ByteBuffer deferredOut, ByteBuffer counters, int flags);   // the same for a flagged step: vote words
     static native long builderCreate(int nGroups, int followers);                                // the event loops' queues: per-group FIFOs -> rows of a step
     static native void builderDestroy(long b);
     static native void builderPushSubmit(long b, int gid, int count, int unavailableMask);       // RaftStub.submit: to the FRONT of the group's queue
@@ -81,5 +86,7 @@ final class NativeEngine {
     static native int  outboxToReplies(ByteBuffer outStruct, int nGroups, int localSlot, ByteBuffer placed, ByteBuffer placedRow, int n, ByteBuffer replyRecsOut);
     static native void requestToCreq(ByteBuffer rec, ByteBuffer entryTerms, int row, long nowMs, boolean hostResult, ByteBuffer cinStruct, int nGroups,
                                      ByteBuffer creqsStruct, int reqCap, int escCap, int entCap);   // a request record -> the compact step's request list
+    static native void requestToCreqEx(ByteBuffer rec, ByteBuffer entryTerms, int row, long nowMs, boolean hostResult, ByteBuffer cinStruct, int nGroups,
+                                       ByteBuffer creqsStruct, int reqCap, int escCap, int entCap, int flags);   // the same for a flagged step: vote records
     static native int  coutboxToReplies(ByteBuffer coutStruct, int nGroups, int localSlot, ByteBuffer placed, ByteBuffer placedRow, int n, ByteBuffer replyRecsOut);
 }

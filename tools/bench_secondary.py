@@ -10,7 +10,9 @@ parity tests replay against the oracle); every step is generator kernel -> step 
 only the step kernel is inside the CUDA-event pairs (second pass over the same stream after a rollback of the tables).  Algorithmic bytes per unit are SURVEY §8(d)'s:
 B_vote = 64, B_ack(R) = 184 + 8(R-2), B_req(n) = 160 + 32 n.  Prints one JSON line per configuration.
 
---e2e instead runs config #5 end to end through the dense host path and the compact one with its request list (run_e2e)."""
+--e2e instead runs config #5 end to end through the dense host path and the compact one with its request list (run_e2e);
+--e2e3 [--groups G] runs config #3 end to end through the dense path, the compact path, and the compact path with
+RAFTING_COMPACT_ELECTIONS (run_e2e3)."""
 import json
 import os
 import sys
@@ -301,9 +303,204 @@ def run_e2e(G=524288, R=3, rows=4, settle=24, window=12, passes=3, seed=0x5EED00
     return rec
 
 
+def run_e2e3(G=262144, R=5, rows=1, settle=4, window=12, passes=3, seed=0x5EED0003, local_slot=2):
+    """config #3 (vote storm, PreVote on) end to end through three host paths.  A window of launches is recorded on the device
+    path; each host path then replays it from pinned caller-owned buffers filled before the clock starts, four launches in
+    flight:
+      dense      rafting_step_begin_host
+      compact    rafting_step_begin_compact_req: every vote reply and ballot an escape record, every vote request an op escape
+      elections  rafting_step_begin_compact_ex(RAFTING_COMPACT_ELECTIONS): replies as ev_c words, ballots as plan_c lanes,
+                 vote requests as records
+    Both compact paths get the escape capacity --e2e uses (rows x G x F / 8 records down); a launch whose escape list overflows
+    it is completed with rafting_step_fetch_dense, and those bytes are counted.  Launch 0 of the window answers ballots of the
+    device path (no tags): it runs once, untimed, and the state after it is where every pass starts.  Every path must end in
+    the device path's state.  Rates are per timed pass (one value per pass)."""
+    import time
+    import torch
+    from rafting_b200 import compact
+    F, NSL, EL = R - 1, 4, abi.COMPACT_ELECTIONS
+    dev = torch.device("cuda:0")
+    L = _bind()
+    # ---- record the window on the device path ----
+    e = engine.Engine(abi.make_cfg(replicas=R, local_slot=local_slot, max_groups=G, max_rows=rows, pre_vote=True,
+                                   entry_pool_cap=workload.POOL_TERMS))
+    e.open_bulk(0, init_array(G, term=1 + np.arange(G) % 5, last_index=100 + np.arange(G) % 50, last_term=1 + np.arange(G) % 5))
+    ib = devbatch.DevInbox(rows, G, F, dev, requests=True)
+    ob = [devbatch.DevOutbox(rows, G, F, G, dev) for _ in range(2)]
+    w = workload.make_wl(seed, rows, G, F, local_slot=local_slot)
+    prev, inboxes = None, []
+    for k in range(settle + window):
+        ic = ib.as_c()
+        assert L.rafting_wl_vote_step(C.byref(w), k, None if prev is None else C.byref(prev), C.byref(ic), 1, C.c_void_p(e.stream())) == 0
+        if k == settle:
+            torch.cuda.synchronize(); e.checkpoint()                      # the state at the start of the window
+        if k >= settle:
+            torch.cuda.synchronize()
+            h = abi.Inbox(rows, G, F, with_ops=False, with_events=False)
+            for name, dt, lane in (("op_meta", np.uint64, 0), ("op_nr", abi.I64X2, 0), ("op_ab", abi.I64X2, 0), ("op_cd", abi.I64X2, 0),
+                                   ("op_e", np.int64, 0), ("ev_meta", np.uint64, 1), ("ev_tn", abi.I64X2, 1), ("ev_el", abi.I64X2, 1)):
+                setattr(h, name, ib.t[name].cpu().numpy().view(dt).reshape((rows, G, F) if lane else (rows, G)))
+            inboxes.append(h)
+        prev = ob[k & 1].as_c()
+        e.step_device(ic, prev, e.stream())
+    torch.cuda.synchronize()
+    digest_dev = e.digest(0, G)
+    del ib, ob
+    e.restore()
+    big = rows * G * (F + 2)                                              # room for every record: the record passes never overflow
+    enc0 = compact.encode_inbox(inboxes[0], None, None, None, elections=True)
+    cout0 = compact.CompactOutbox(rows, G, F, esc_cap=big)
+    e.step_compact(enc0, cout0, reqs=enc0.reqs, flags=EL)                # launch 0, untimed
+    e.checkpoint()
+    ESC_CAP = rows * G * F // 8
+    n = window - 1
+    units = {"vote_replies": 0, "vote_requests": 0}
+    for h in inboxes[1:]:
+        evk = (h.ev_meta & np.uint64(0xF)).astype(np.int64)
+        opk = (h.op_meta & np.uint64(0xFF)).astype(np.int64)
+        units["vote_replies"] += int(((evk == abi.EV_PV_REPLY) | (evk == abi.EV_RV_REPLY)).sum())
+        units["vote_requests"] += int(((opk == abi.OP_PREVOTE_REQ) | (opk == abi.OP_VOTE_REQ)).sum())
+    keep = []                                                             # pinned blocks stay alive until the end
+
+    def pinned(nbytes):
+        t = torch.zeros(max(1, int(nbytes)), dtype=torch.uint8).pin_memory(); keep.append(t)
+        return t.numpy()
+
+    def dense_outbox():
+        o = devbatch.DevOutbox(rows, G, F, G, "cpu")
+        cols = {name: t.pin_memory() for name, t in o.t.items()}
+        keep.extend(cols.values())
+        oc = abi.OutboxC()
+        for name, t in cols.items():
+            setattr(oc, name, t.data_ptr())
+        return oc, sum(t.numel() for t in cols.values())
+
+    # ---- record passes (untimed) of the two compact paths: the inputs as a pump builds them, the tags the engine hands out ----
+    _, out_off = engine.Engine.compact_layout(rows, G, F, 0, ESC_CAP)
+    down_cols = int(out_off[10])
+    dense_down = dense_outbox()[1]
+    recorded = {}
+    for path, flags in (("compact", 0), ("elections", EL)):
+        e.restore()
+        nxt = None
+        if flags:
+            d0 = compact.decode_outbox(cout0, elections=True)
+            nxt = dict(tags=cout0.tags(rpc_only=True), sent_term=cout0.current_term.copy(), sent_inc=cout0.incarnation.copy(),
+                       ballot_term=d0.ballot_term.copy(), ballot_inc=d0.ballot_meta >> np.uint64(32), ballot_tags=cout0.ballot_tags())
+        cins, reqs, up, down, esc_ev, esc_op, esc_out, fallbacks = [], [], [], [], [], [], [], 0
+        for k in range(1, window):
+            if flags:
+                ci = compact.encode_inbox(inboxes[k], nxt["tags"], nxt["sent_term"], nxt["sent_inc"], elections=True,
+                                          ballot_term=nxt["ballot_term"], ballot_inc=nxt["ballot_inc"], ballot_tags=nxt["ballot_tags"])
+            else:
+                ci = compact.encode_inbox(inboxes[k], None, None, None)
+            q = ci.reqs if ci.reqs is not None else compact.CompactRequests()
+            in_off, _ = engine.Engine.compact_layout(rows, G, F, len(ci.esc), ESC_CAP)
+            ci = compact.inbox_in_block(pinned(in_off[5]), in_off, ci)
+            r_off = engine.Engine.compact_req_layout(len(q.req), len(q.op_esc), len(q.ent_terms))
+            blk = pinned(r_off[3])
+            views = []
+            for a, off in ((q.req, r_off[0]), (q.op_esc, r_off[1]), (q.ent_terms, r_off[2])):
+                v = blk[int(off):int(off) + a.nbytes].view(a.dtype)
+                v[...] = a
+                views.append(v)
+            q = compact.CompactRequests(*views)
+            co = compact.CompactOutbox(rows, G, F, esc_cap=big)
+            e.step_compact(ci, co, reqs=q, flags=flags)
+            cins.append(ci.as_c()); reqs.append(q.as_c())
+            n_out = int(co.counts[0])
+            span = (in_off[4] + len(ci.esc) * abi.CESC_IN.itemsize) if len(ci.esc) else (in_off[3] + ci.ev_c.nbytes)
+            up.append(span + (int(r_off[3]) if len(q.req) or len(q.op_esc) else 0))
+            over = n_out > ESC_CAP
+            fallbacks += over
+            down.append(down_cols + max(min(n_out, ESC_CAP), min(256, ESC_CAP)) * abi.CESC_OUT.itemsize + (dense_down if over else 0))
+            esc_ev.append(len(ci.esc)); esc_op.append(len(q.op_esc)); esc_out.append(n_out)
+            if flags:
+                d = compact.decode_outbox(co, elections=True)
+                nxt = dict(tags=co.tags(rpc_only=True), sent_term=co.current_term.copy(), sent_inc=co.incarnation.copy(),
+                           ballot_term=d.ballot_term.copy(), ballot_inc=d.ballot_meta >> np.uint64(32), ballot_tags=co.ballot_tags())
+        recorded[path] = dict(cins=cins, reqs=reqs, flags=flags, exact=bool((e.digest(0, G) == digest_dev).all()),
+                              stats={"h2d_bytes_per_launch": int(np.mean(up)), "d2h_bytes_per_launch": int(np.mean(down)),
+                                     "escape_records_in_per_launch": {"events": float(np.mean(esc_ev)), "ops": float(np.mean(esc_op))},
+                                     "escape_records_out_per_launch": float(np.mean(esc_out)),
+                                     "dense_fallbacks_per_launch": fallbacks / n})
+    # ---- the pinned buffers of the timed passes ----
+    couts, fall = [], []
+    for sl in range(NSL):
+        couts.append(compact.outbox_in_block(pinned(out_off[11]), out_off, rows, G, F, ESC_CAP))
+        fall.append(dense_outbox()[0])
+    cout_c = [co.as_c() for co in couts]
+    host_in = []
+    for k in range(1, window):
+        h = inboxes[k]
+        cols = {name: torch.from_numpy(np.ascontiguousarray(getattr(h, name)).view(np.uint8).reshape(-1)).pin_memory()
+                for name in ("op_meta", "op_nr", "op_ab", "op_cd", "op_e", "ev_meta", "ev_tn", "ev_el")}
+        ic = abi.InboxC()
+        ic.rows, ic.n_active, ic.flags, ic.ent_count = rows, 0, 0, 0
+        for name, t in cols.items():
+            setattr(ic, name, t.data_ptr())
+        host_in.append((cols, ic))
+    host_out = [dense_outbox() for _ in range(NSL)]
+    up_d = sum(t.numel() for t in host_in[0][0].values())
+
+    def dense_pass():
+        for j in range(n):
+            sl = j % NSL
+            if j >= NSL:
+                e.step_wait_slot(sl)
+            e.step_begin_host(sl, host_in[j][1], host_out[sl][0])
+        for sl in range(NSL):
+            e.step_wait_slot(sl)
+
+    def compact_pass(path):
+        rec = recorded[path]
+
+        def finish(sl):
+            e.step_wait_compact(sl)
+            if int(couts[sl].counts[0]) > ESC_CAP:                        # the escape list overflowed: the lossless fallback
+                e.step_fetch_dense(sl, fall[sl])
+        for j in range(n):
+            sl = j % NSL
+            if j >= NSL:
+                finish(sl)
+            e.step_begin_compact_ex(sl, rec["cins"][j], rec["reqs"][j], cout_c[sl], rec["flags"])
+        for sl in range(NSL):
+            finish(sl)
+
+    res = {}
+    for name, fn in (("dense", dense_pass), ("compact", lambda: compact_pass("compact")), ("elections", lambda: compact_pass("elections"))):
+        e.restore(); fn()                                                 # untimed: every slot's staging exists before the clock
+        exact = bool((e.digest(0, G) == digest_dev).all())
+        rates = []
+        for _ in range(passes):
+            e.restore()
+            t0 = time.perf_counter()
+            fn()
+            spent = time.perf_counter() - t0
+            rates.append(spent)
+            exact = exact and bool((e.digest(0, G) == digest_dev).all())
+        res[name] = {"vote_replies_per_s": [units["vote_replies"] / s for s in rates],
+                     "vote_requests_per_s": [units["vote_requests"] / s for s in rates],
+                     "launches_per_pass": n, "end_state_equals_device_path": exact}
+    res["dense"].update({"path": "rafting_step_begin_host", "h2d_bytes_per_launch": int(up_d), "d2h_bytes_per_launch": int(host_out[0][1] + 16)})
+    res["compact"].update({"path": "rafting_step_begin_compact_req", **recorded["compact"]["stats"],
+                           "record_pass_exact": recorded["compact"]["exact"]})
+    res["elections"].update({"path": "rafting_step_begin_compact_ex(RAFTING_COMPACT_ELECTIONS)", **recorded["elections"]["stats"],
+                             "record_pass_exact": recorded["elections"]["exact"]})
+    rec = {"config": "config3_e2e", "groups": G, "replicas": R, "rows_per_launch": rows, "window_launches": n, "passes": passes,
+           "launches_in_flight": NSL, "escape_cap_down": ESC_CAP,
+           "units_per_launch": {k: v / n for k, v in units.items()}, "card": card(), **res}
+    print(json.dumps(rec), flush=True)
+    e.close()
+    return rec
+
+
 def main():
     if "--e2e" in sys.argv[1:]:
         run_e2e()
+    elif "--e2e3" in sys.argv[1:]:
+        a = sys.argv[1:]
+        run_e2e3(G=int(a[a.index("--groups") + 1]) if "--groups" in a else 262144)
     else:
         run_all()
 
