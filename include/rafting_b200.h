@@ -587,6 +587,23 @@ int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot /* 0..3 */
 #define RAFTING_CREQ_VOTE_PRE 1u
 #define RAFTING_CREQ_VOTE_RV  2u
 #define RAFTING_CREQ_VOTE(m)  (((uint32_t)(m) >> 11) & 3u)
+/* PREV_TERM on the compact path (flag RAFTING_COMPACT_PREV_TERM of rafting_step_begin_compact_ex; it combines freely with
+ * RAFTING_COMPACT_ELECTIONS, so flags is 0, 1, 4 or 5, and every other bit is refused).  The first heartbeats of a newly
+ * elected leader, and AppendEntries that follow an older term or catch a follower up after a rejection, carry a prevLogTerm
+ * below the group's term: under kind 1 each is a RAFTING_CESC_PLAN record.  Under the flag such a plan is one plan_c word:
+ *        bits 0..2 RAFTING_CPLAN_AE_PREV_TERM (7) | 3 heartbeat | 4 zero (an escaped AE keeps kind 1) | 5..10 tag (as kind 1) |
+ *        11..16 count | 17..24 dprev | 25..27 dterm - 1 | 28..31 dcommit
+ *     prevLogIndex = last_entry[g].x - dprev      prevLogTerm  = current_term[g] - dterm      (dterm 1..8)
+ *     lastIndex    = prevLogIndex + count         leaderCommit = commit_index[g] - dcommit    (dcommit 0..15)
+ *     epochAtSend  = epoch[g].x                   incarnation  = incarnation[g]               (end-of-step columns, as kind 1)
+ *   It is used only when every other kind-1 condition holds (incarnation, epochAtSend, lastIndex == prevLogIndex + count,
+ *   count < 64, dprev < 256), 1 <= current_term[g] - prevLogTerm <= 8 and dcommit < 16.  A plan that fits kind 1 stays kind
+ *   1; any other plan stays a RAFTING_CESC_PLAN record.  The plan takes its tag and parks (epochAtSend, lastIndex) and the
+ *   incarnation exactly as kind 1 does, so its ack or failure is an ordinary AE ev_c word: nothing else of the step changes. */
+#define RAFTING_COMPACT_PREV_TERM 4u
+#define RAFTING_CPLAN_AE_PREV_TERM 7u
+#define RAFTING_CPLAN_DTERM(w)    ((((uint32_t)(w) >> 25) & 7u) + 1u)    /* current_term[g] - prevLogTerm, 1..8 */
+#define RAFTING_CPLAN_DCOMMIT7(w) (((uint32_t)(w) >> 28) & 15u)           /* the dcommit of a kind-7 word */
 int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot /* 0..3 */, const rafting_cinbox_t* in_host,
                                   const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host, uint32_t flags);
 int rafting_step_wait_compact (rafting_engine_t* e, uint32_t slot);

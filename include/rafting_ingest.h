@@ -199,6 +199,18 @@ int rafting_request_to_creq(const rafting_req_rec_t* r, const int64_t* entry_ter
  * RAFTING_CESC_REPLY escape record.  RAFTING_E_CAPACITY when the escape list overflowed (fetch the dense outbox instead). */
 int rafting_coutbox_to_replies(const rafting_coutbox_t* co, uint32_t n_groups, uint32_t local_slot, const rafting_req_rec_t* placed,
                                const uint8_t* placed_row, uint32_t n, rafting_batch_rec_t* out, uint32_t* n_out);
+/* rafting_outbox_to_requests over a waited-for compact outbox of a step begun with `flags` (RAFTING_COMPACT_ELECTIONS /
+ * RAFTING_COMPACT_PREV_TERM, or 0): the same records, in the same order, that rafting_outbox_to_requests emits for the dense
+ * outbox the compact one stands for, with the same incarnation -> term memory in d.  Plans come from their plan_c words (kind
+ * 7 under RAFTING_COMPACT_PREV_TERM) or their RAFTING_CESC_PLAN records, ballots from their lanes' words (under
+ * RAFTING_COMPACT_ELECTIONS) or their RAFTING_CESC_BALLOT records; escape records are matched by slot, whatever their order.
+ * tags[i] is the tag the pump puts into the pending entry of out[i] (rafting_pending_put): the plan's tag for an AE / IS, the
+ * lane's tag for a compact ballot, RAFTING_CTAG_NONE for an escaped ballot or an untagged plan.  out and tags have room for
+ * cap records (RAFTING_E_CAPACITY beyond).  RAFTING_E_CAPACITY too when the escape list overflowed (counts[0] > esc_cap):
+ * fetch the dense outbox and use rafting_outbox_to_requests.  RAFTING_E_INVAL: an unknown flag, or an escaped plan word
+ * without its record. */
+int rafting_coutbox_to_requests(rafting_dispatch_t* d, const rafting_coutbox_t* co, uint32_t rows, uint32_t flags,
+                                rafting_req_rec_t* out, uint8_t* tags, uint32_t cap, uint32_t* n_out, uint32_t* n_unknown);
 
 /* ---- replies -> compact wire words (the compact host path of include/rafting_b200.h) -------------------------------------
  * The pending-invocation table of the pump: what NettyNode keeps per connection as (scope, sequence) -> Invocation
@@ -231,7 +243,8 @@ int rafting_failures_to_cinbox(rafting_pending_t* p, uint32_t peer, const int32_
                                uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred, uint32_t* n_deferred, uint32_t* n_unknown);
 
 /* The same three writers for a step begun with RAFTING_COMPACT_ELECTIONS (rafting_step_begin_compact_ex); flags == 0 is exactly
- * the function without _ex.  Under the flag:
+ * the function without _ex.  They accept RAFTING_COMPACT_PREV_TERM and ignore it (an ack to a kind-7 plan is an ordinary AE
+ * ack), so that a pump passes one flags word everywhere.  Under RAFTING_COMPACT_ELECTIONS:
  *   rafting_request_to_creq_ex  a PreVote / RequestVote with src_slot < 32, 0 <= now - row_base[row] <= 65535 and
  *                               0 <= term - lastLogTerm < 2^32 becomes a vote record (no entries, d_commit 0)
  *   rafting_acks_to_cinbox_ex   a vote reply whose pending entry has a tag (the ballot lane's, put with term = the ballot

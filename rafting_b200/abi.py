@@ -366,6 +366,11 @@ def cev_vote_make(kind: int, outcome: int, granted: int, tag: int, c: int, dt: i
     return kind | (outcome << 4) | ((1 if granted else 0) << 6) | ((tag & 0x1F) << 8) | ((c & 7) << 13) | ((dt & 0xFFFF) << 16)
 
 
+# AE plans whose prevLogTerm lies 1..8 below the group's term as plan_c words (rafting_step_begin_compact_ex flag)
+COMPACT_PREV_TERM = 4
+CPLAN_AE_PREV_TERM = 7
+
+
 class CReqsC(C.Structure):
     _fields_ = [("n_req", C.c_uint32), ("n_op_esc", C.c_uint32), ("req", C.c_void_p), ("op_esc", C.c_void_p),
                 ("ent_terms", C.c_void_p), ("ent_count", C.c_uint32), ("req_entries", C.c_uint32)]

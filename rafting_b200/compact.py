@@ -92,11 +92,11 @@ class CompactOutbox:
     def tags(self, rpc_only: bool = False) -> np.ndarray:
         """tag of every plan, [rows, n, F] (abi.CTAG_NONE = none).  rpc_only: CTAG_NONE on every lane that holds no AE / IS
         plan, so that every tag names an AppendEntries / InstallSnapshot in flight (what encode_inbox(elections=True) needs
-        for acks: its escaped words free their tag)."""
+        for acks: its escaped words free their tag).  A kind-7 word (abi.COMPACT_PREV_TERM) is an AppendEntries."""
         t = ((self.plan_c >> np.uint32(5)) & np.uint32(63)).astype(np.uint8)
         if rpc_only:
             k = self.plan_c & np.uint32(7)
-            t[(k != abi.PLAN_AE) & (k != abi.PLAN_IS)] = abi.CTAG_NONE
+            t[(k != abi.PLAN_AE) & (k != abi.PLAN_IS) & (k != abi.CPLAN_AE_PREV_TERM)] = abi.CTAG_NONE
         return t
 
     def ballot_tags(self) -> np.ndarray:
@@ -285,15 +285,19 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     return c
 
 
-def decode_outbox(co: CompactOutbox, G: int | None = None, elections: bool = False) -> abi.Outbox:
+def decode_outbox(co: CompactOutbox, G: int | None = None, elections: bool = False, prev_term: bool = False) -> abi.Outbox:
     """The dense outbox a compact step stands for (rep_term / ballots / escaped plans come from the escape list).
-    elections: the step was begun with abi.COMPACT_ELECTIONS, so plan_c lanes of kind CPLAN_PREVOTE / CPLAN_VOTE are ballots."""
+    elections: the step was begun with abi.COMPACT_ELECTIONS, so plan_c lanes of kind CPLAN_PREVOTE / CPLAN_VOTE are ballots.
+    prev_term: the step was begun with abi.COMPACT_PREV_TERM, so a lane of kind CPLAN_AE_PREV_TERM is an AE plan whose
+    prevLogTerm lies dterm below the group's term."""
     rows, n, F = co.rows, co.n, co.F
     if int(co.counts[0]) > co.esc_cap:
         raise OverflowError("escape list overflow: fetch the dense outbox (rafting_step_fetch_dense)")
     o = abi.Outbox(rows, n, F, n if G is None else G)
     pc = co.plan_c.astype(np.uint64)
     kind = (pc & U64(7)).astype(np.int64)
+    older = (kind == abi.CPLAN_AE_PREV_TERM) if prev_term else np.zeros(kind.shape, bool)
+    kind = np.where(older, abi.PLAN_AE, kind)
     if elections and F:
         bk = kind[:, :, 0]                                                       # every lane of a compact ballot has the word
         pre, vote = bk == abi.CPLAN_PREVOTE, bk == abi.CPLAN_VOTE
@@ -308,7 +312,8 @@ def decode_outbox(co: CompactOutbox, G: int | None = None, elections: bool = Fal
     esc = ((pc >> U64(4)) & U64(1)) != 0
     cnt = ((pc >> U64(11)) & U64(63)).astype(np.int64)
     dprev = ((pc >> U64(17)) & U64(255)).astype(np.int64)
-    dcommit = ((pc >> U64(25)) & U64(127)).astype(np.int64)
+    dcommit = np.where(older, (pc >> U64(28)) & U64(15), (pc >> U64(25)) & U64(127)).astype(np.int64)
+    dterm = np.where(older, ((pc >> U64(25)) & U64(7)) + U64(1), U64(0)).astype(np.int64)
     # a compact plan was sent by the role object that holds the group at the end of the step
     o.plan_meta[:] = np.where(kind != 0, kind.astype(np.uint64) | (hb << U64(4)) | (cnt.astype(np.uint64) << U64(16)) |
                               (co.incarnation.astype(np.uint64)[None, :, None] << U64(32)), U64(0))
@@ -317,7 +322,7 @@ def decode_outbox(co: CompactOutbox, G: int | None = None, elections: bool = Fal
     ae, isn = (kind == abi.PLAN_AE) & ~esc, (kind == abi.PLAN_IS) & ~esc
     prev = last_x - dprev
     o.plan_pp["x"] = np.where(ae, prev, np.where(isn, ep["x"][None, :, None], 0))
-    o.plan_pp["y"] = np.where(ae, term, np.where(isn, ep["y"][None, :, None], 0))
+    o.plan_pp["y"] = np.where(ae, term - dterm, np.where(isn, ep["y"][None, :, None], 0))
     o.plan_lc["x"] = np.where(ae, prev + cnt, np.where(isn, ep["x"][None, :, None], 0))
     o.plan_lc["y"] = np.where(ae | isn, commit - dcommit, 0)
     o.plan_epoch[:] = np.where(kind != 0, ep["x"][None, :, None], 0)

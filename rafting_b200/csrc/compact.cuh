@@ -9,7 +9,9 @@
 //                   incarnation in the table; whatever breaks a compact rule goes, in full, to the escape list
 //
 // Under RAFTING_COMPACT_ELECTIONS (the EL instantiations) vote RPCs take tags as well: a compact ballot's lanes park
-// (ballot term, 0) and the asking role's incarnation, and a vote reply word gets them back.
+// (ballot term, 0) and the asking role's incarnation, and a vote reply word gets them back.  Under RAFTING_COMPACT_PREV_TERM
+// (the PT instantiations of pack_kernel) an AE plan whose prevLogTerm lies 1..8 below the group's term travels as a kind-7
+// word instead of an escape record; it takes and parks its tag as a kind-1 plan does, so its ack is an ordinary AE word.
 //
 // One thread per (group, follower) walks the rows in order in both kernels, so the tag bitmap of a lane is only ever touched
 // by its own thread, and the three kernels of a step (unpack, step, pack) are ordered on the engine's stream.  What this
@@ -233,7 +235,8 @@ __device__ __forceinline__ uint32_t ballot_lane_word(const OutboxD& in, size_t g
     return bk | (tag << 5);
 }
 
-template <bool EL>
+// PT: steps begun with RAFTING_COMPACT_PREV_TERM (an AE plan that breaks only the prevLogTerm rule becomes a kind-7 word)
+template <bool EL, bool PT>
 __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, OutboxD in, COutD out, i64x2* __restrict__ table, uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits) {
     const uint32_t GF = T.G * T.F;
     const uint32_t t = blockIdx.x * 256u + threadIdx.x;
@@ -267,14 +270,22 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
                 const uint64_t dcommit = (uint64_t)commit_end - (uint64_t)lc.y;
                 uint64_t dprev = 0;
                 bool fits = pe == epoch_end.x && RAFTING_PLM_INC(pm) == inc_end && count < 64u;
+                [[maybe_unused]] bool older = false;                                // PT: fits kind 7 (then never kind 1)
+                [[maybe_unused]] uint64_t gap = 0;                                  // PT: current_term - prevLogTerm
                 if (kind == RAFTING_PLAN_AE) {
                     dprev = (uint64_t)last_end.x - (uint64_t)pp.x;
+                    if constexpr (PT) {
+                        gap = (uint64_t)term_end - (uint64_t)pp.y;
+                        older = fits && gap - 1u < 8u && lc.x == (int64_t)((uint64_t)pp.x + count) && dprev < 256u && dcommit < 16u;
+                    }
                     fits = fits && pp.y == term_end && lc.x == (int64_t)((uint64_t)pp.x + count) && dprev < 256u && dcommit < 128u;
                 } else if (kind == RAFTING_PLAN_IS) {
                     fits = fits && pp.x == epoch_end.x && pp.y == epoch_end.y && lc.x == epoch_end.x && dcommit < 128u;
                 } else fits = fits && pp.x == 0 && pp.y == 0 && lc.x == 0 && lc.y == 0;
                 pc = kind | ((uint32_t)RAFTING_PLM_HB(pm) << 3) | (tag << 5);
                 if (fits) pc |= (count << 11) | ((uint32_t)dprev << 17) | ((kind == RAFTING_PLAN_AE || kind == RAFTING_PLAN_IS) ? ((uint32_t)dcommit << 25) : 0u);
+                else if (PT && older)
+                    pc |= RAFTING_CPLAN_AE_PREV_TERM | (count << 11) | ((uint32_t)dprev << 17) | ((uint32_t)(gap - 1u) << 25) | ((uint32_t)dcommit << 28);
                 else { pc |= 1u << 4; put_escape(out, RAFTING_CESC_PLAN, (uint32_t)idx, pm | ((uint64_t)(tag == RAFTING_CTAG_NONE ? 255u : tag) << 8), pp.x, pp.y, lc.x, lc.y, pe); }
             }
             out.plan_c[idx] = pc;
@@ -399,8 +410,8 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
                                              const rafting_coutbox_t* out, uint32_t flags) {
     using namespace rafting;
     if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
-    if (flags & ~RAFTING_COMPACT_ELECTIONS) return fail(RAFTING_E_INVAL, "unknown compact step flags 0x%x", flags);
-    const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0;
+    if (flags & ~(RAFTING_COMPACT_ELECTIONS | RAFTING_COMPACT_PREV_TERM)) return fail(RAFTING_E_INVAL, "unknown compact step flags 0x%x", flags);
+    const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0, pt = (flags & RAFTING_COMPACT_PREV_TERM) != 0;
     const bool has_reqs = reqs && (reqs->n_req || reqs->n_op_esc);
     if (!in->row_base || (!in->op_c && !in->ev_c && !has_reqs))
         return fail(RAFTING_E_INVAL, "compact inbox needs row_base and at least one of op_c / ev_c / a request");
@@ -534,8 +545,8 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
     CU(cudaGetLastError());
     rc = launch_step(e, di, dov, e->stream);
     if (rc) { cudaStreamSynchronize(H->s_h2d); return rc; }
-    if (el) pack_kernel<true><<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits);
-    else pack_kernel<false><<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits);
+    auto* pack = el ? (pt ? pack_kernel<true, true> : pack_kernel<true, false>) : (pt ? pack_kernel<false, true> : pack_kernel<false, false>);
+    pack<<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits);
     CU(cudaGetLastError());
     CU(cudaEventRecord(S.ev_kernel, e->stream));
     // ---- D2H: every wire column + the counters; the escape list only when the counters say it holds something ----

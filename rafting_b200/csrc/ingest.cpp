@@ -9,6 +9,8 @@
 
 namespace {
 constexpr uint8_t SOH = 0x01, STX = 0x02, ETX = 0x03, EOT = 0x04;          // EventCodec.java:29-32
+// every flag a compact step may carry: a pump passes one flags word to every compact writer and reader
+constexpr uint32_t COMPACT_FLAGS = RAFTING_COMPACT_ELECTIONS | RAFTING_COMPACT_PREV_TERM;
 inline uint32_t be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
 inline void put_be32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v; }
 }  // namespace
@@ -435,7 +437,7 @@ extern "C" int rafting_request_to_creq_ex(const rafting_req_rec_t* r, const int6
                                           int host_result, const rafting_cinbox_t* in, uint32_t n_groups, rafting_creqs_t* q,
                                           uint32_t req_cap, uint32_t esc_cap, uint32_t ent_cap, uint32_t flags) {
     if (!r || !in || !in->row_base || !q || (q->n_req && !q->req) || (q->n_op_esc && !q->op_esc)) return RAFTING_E_INVAL;
-    if (flags & ~RAFTING_COMPACT_ELECTIONS) return RAFTING_E_INVAL;
+    if (flags & ~COMPACT_FLAGS) return RAFTING_E_INVAL;
     if (r->gid >= n_groups || row >= in->rows) return RAFTING_E_INVAL;
     if (r->kind != RAFTING_OP_AE_REQUEST && r->kind != RAFTING_OP_PREVOTE_REQ && r->kind != RAFTING_OP_VOTE_REQ &&
         r->kind != RAFTING_OP_IS_REQUEST) return RAFTING_E_INVAL;
@@ -522,6 +524,102 @@ extern "C" int rafting_coutbox_to_replies(const rafting_coutbox_t* co, uint32_t 
         out[k++] = r;
     }
     *n_out = k;
+    return RAFTING_OK;
+}
+
+// rafting_outbox_to_requests over a waited-for compact outbox, without decoding it into dense columns first: the plan of a
+// lane comes from its plan_c word or, when escaped, from its escape record; a ballot from its lanes' words (flagged) or its
+// escape record.  The escape list is filled through one atomic counter, so its records are found by slot, not by position.
+extern "C" int rafting_coutbox_to_requests(rafting_dispatch_t* d, const rafting_coutbox_t* co, uint32_t rows, uint32_t flags,
+                                           rafting_req_rec_t* out, uint8_t* tags, uint32_t cap, uint32_t* n_out, uint32_t* n_unknown) {
+    if (!d || !co || !out || !tags || !n_out || !co->plan_c || !co->commit_index || !co->current_term || !co->incarnation ||
+        !co->last_entry || !co->epoch || !co->counts || (flags & ~COMPACT_FLAGS)) return RAFTING_E_INVAL;
+    if (co->counts[0] > co->esc_cap) return RAFTING_E_CAPACITY;               // the escape list overflowed: use the dense outbox
+    if (co->counts[0] && !co->esc) return RAFTING_E_INVAL;
+    const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0, pt = (flags & RAFTING_COMPACT_PREV_TERM) != 0;
+    const uint32_t G = d->G, F = d->F;
+    for (uint32_t g = 0; g < G; g++) d->learn(g, co->incarnation[g], co->current_term[g]);
+    std::vector<std::pair<uint32_t, uint32_t>> pesc, besc;                   // (slot, index) of the plan / ballot escapes, sorted
+    for (uint32_t k = 0; k < co->counts[0]; k++) {
+        if (co->esc[k].kind == RAFTING_CESC_PLAN) pesc.push_back({co->esc[k].slot, k});
+        else if (co->esc[k].kind == RAFTING_CESC_BALLOT) besc.push_back({co->esc[k].slot, k});
+    }
+    std::sort(pesc.begin(), pesc.end());
+    std::sort(besc.begin(), besc.end());
+    auto find = [](const std::vector<std::pair<uint32_t, uint32_t>>& v, size_t slot) -> int64_t {
+        const auto it = std::lower_bound(v.begin(), v.end(), std::make_pair((uint32_t)slot, 0u));
+        return it != v.end() && it->first == slot ? (int64_t)it->second : -1;
+    };
+    uint32_t n = 0, unknown = 0;
+    auto slot_of = [&](uint32_t lane) { return (uint8_t)(lane < d->slot ? lane : lane + 1); };
+    for (uint32_t r = 0; r < rows; r++) {
+        for (uint32_t g = 0; g < G; g++)
+            for (uint32_t f = 0; f < F; f++) {
+                const size_t li = ((size_t)r * G + g) * F + f;
+                const uint32_t w = co->plan_c[li], wk = RAFTING_CPLAN_KIND(w);
+                const bool older = pt && wk == RAFTING_CPLAN_AE_PREV_TERM;
+                uint32_t kind = older ? RAFTING_PLAN_AE : wk, inc = co->incarnation[g], count = 0;
+                int64_t a = 0, b = 0, last = 0, commit = 0, epoch = co->epoch[g].x;
+                if (kind != RAFTING_PLAN_AE && kind != RAFTING_PLAN_IS) continue;   // a ballot lane, or a plan that sends nothing
+                if (!older && RAFTING_CPLAN_ESCAPED(w)) {
+                    const int64_t k = find(pesc, li);
+                    if (k < 0) return RAFTING_E_INVAL;                      // an escaped plan without its record
+                    const rafting_cesc_out_t& e = co->esc[k];
+                    kind = RAFTING_PLM_KIND(e.meta); inc = RAFTING_PLM_INC(e.meta); count = RAFTING_PLM_COUNT(e.meta);
+                    a = e.a; b = e.b; last = e.c; commit = e.d; epoch = e.e;
+                    if (kind != RAFTING_PLAN_AE && kind != RAFTING_PLAN_IS) continue;
+                } else if (kind == RAFTING_PLAN_AE) {
+                    count = RAFTING_CPLAN_COUNT(w);
+                    a = (int64_t)((uint64_t)co->last_entry[g].x - RAFTING_CPLAN_DPREV(w));
+                    b = older ? (int64_t)((uint64_t)co->current_term[g] - RAFTING_CPLAN_DTERM(w)) : co->current_term[g];
+                    last = (int64_t)((uint64_t)a + count);
+                    commit = (int64_t)((uint64_t)co->commit_index[g] - (older ? RAFTING_CPLAN_DCOMMIT7(w) : RAFTING_CPLAN_DCOMMIT(w)));
+                } else {
+                    a = co->epoch[g].x; b = co->epoch[g].y; last = co->epoch[g].x;
+                }
+                const int64_t* t = d->find(g, inc);
+                if (!t) { unknown++; continue; }
+                if (n >= cap) { *n_out = n; if (n_unknown) *n_unknown = unknown; return RAFTING_E_CAPACITY; }
+                rafting_req_rec_t q{};
+                q.gid = g; q.kind = kind == RAFTING_PLAN_AE ? RAFTING_OP_AE_REQUEST : RAFTING_OP_IS_REQUEST;
+                q.src_slot = (uint8_t)d->slot; q.dst_slot = slot_of(f); q.row = (uint8_t)r;
+                q.incarnation = inc; q.count = kind == RAFTING_PLAN_AE ? count : 0;
+                q.term = *t; q.a = a; q.b = b; q.last = last; q.commit = kind == RAFTING_PLAN_AE ? commit : 0; q.epoch = epoch;
+                tags[n] = (uint8_t)RAFTING_CPLAN_TAG(w);
+                out[n++] = q;
+            }
+        for (uint32_t g = 0; g < G; g++) {
+            const size_t gi = (size_t)r * G + g;
+            uint64_t bm = 0; int64_t term = 0; rafting_i64x2_t bl = {0, 0};
+            bool lanes = false;                                              // a compact ballot: its lanes carry the tags
+            const int64_t k = find(besc, gi);
+            if (k >= 0) {
+                const rafting_cesc_out_t& e = co->esc[k];
+                bm = e.meta; term = e.a; bl.x = e.b; bl.y = e.c;
+            } else if (el && F) {
+                const uint32_t bk = RAFTING_CPLAN_KIND(co->plan_c[gi * F]);
+                if (bk == RAFTING_CPLAN_PREVOTE || bk == RAFTING_CPLAN_VOTE) {
+                    const bool pre = bk == RAFTING_CPLAN_PREVOTE;
+                    bm = (pre ? RAFTING_BALLOT_PREVOTE : RAFTING_BALLOT_VOTE) | ((uint64_t)co->incarnation[g] << 32);
+                    term = (int64_t)((uint64_t)co->current_term[g] + (pre ? 1u : 0u)); bl = co->last_entry[g];
+                    lanes = true;
+                }
+            }
+            const uint32_t kind = (uint32_t)(bm & 0xFu);
+            if (kind == RAFTING_BALLOT_NONE) continue;
+            for (uint32_t f = 0; f < F; f++) {
+                if (n >= cap) { *n_out = n; if (n_unknown) *n_unknown = unknown; return RAFTING_E_CAPACITY; }
+                rafting_req_rec_t q{};
+                q.gid = g; q.kind = kind == RAFTING_BALLOT_PREVOTE ? RAFTING_OP_PREVOTE_REQ : RAFTING_OP_VOTE_REQ;
+                q.src_slot = (uint8_t)d->slot; q.dst_slot = slot_of(f); q.row = (uint8_t)r;
+                q.incarnation = (uint32_t)(bm >> 32);
+                q.term = term; q.a = bl.x; q.b = bl.y;
+                tags[n] = (uint8_t)(lanes ? RAFTING_CPLAN_TAG(co->plan_c[gi * F + f]) : RAFTING_CTAG_NONE);
+                out[n++] = q;
+            }
+        }
+    }
+    *n_out = n; if (n_unknown) *n_unknown = unknown;
     return RAFTING_OK;
 }
 
@@ -631,7 +729,7 @@ extern "C" int rafting_acks_to_cinbox_ex(rafting_pending_t* p, uint32_t peer, co
                                          uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred, uint32_t* n_deferred, uint32_t* n_unknown,
                                          uint32_t flags) {
     if (!p || (!acks && n) || !cin || !cin->ev_c || !cin->row_base || !n_esc || !n_deferred || (!deferred && n) || row >= cin->rows ||
-        (flags & ~RAFTING_COMPACT_ELECTIONS))
+        (flags & ~COMPACT_FLAGS))
         return RAFTING_E_INVAL;
     const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0;
     uint32_t* ev = const_cast<uint32_t*>(cin->ev_c);
@@ -685,7 +783,7 @@ extern "C" int rafting_failures_to_cinbox_ex(rafting_pending_t* p, uint32_t peer
                                              rafting_cesc_in_t* esc, uint32_t esc_cap, uint32_t* n_esc, uint32_t* deferred,
                                              uint32_t* n_deferred, uint32_t* n_unknown, uint32_t flags) {
     if (!p || (!sequences && n) || !cin || !cin->ev_c || !cin->row_base || !n_esc || !n_deferred || (!deferred && n) || row >= cin->rows ||
-        (outcome != RAFTING_OUT_ERROR && outcome != RAFTING_OUT_CANCELED) || (flags & ~RAFTING_COMPACT_ELECTIONS)) return RAFTING_E_INVAL;
+        (outcome != RAFTING_OUT_ERROR && outcome != RAFTING_OUT_CANCELED) || (flags & ~COMPACT_FLAGS)) return RAFTING_E_INVAL;
     const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0;
     uint32_t* ev = const_cast<uint32_t*>(cin->ev_c);
     const int64_t dt = now_ms - cin->row_base[row];

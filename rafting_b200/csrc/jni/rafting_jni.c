@@ -256,6 +256,14 @@ JNIEXPORT jint JNICALL FN(outboxToRequests)(JNIEnv* env, jclass k, jlong d, jobj
                                      (rafting_req_rec_t*)BUF(recsOut), (uint32_t)cap, &n, &unknown));
     return (jint)n;
 }
+/* the same over a waited-for compact outbox of a step begun with `flags`; tagsOut gets the pending entry's tag per record */
+JNIEXPORT jint JNICALL FN(coutboxToRequests)(JNIEnv* env, jclass k, jlong d, jobject coutStruct, jint rows, jint flags, jobject recsOut,
+                                             jobject tagsOut, jint cap) {
+    uint32_t n = 0, unknown = 0;
+    CHECK(rafting_coutbox_to_requests((rafting_dispatch_t*)(intptr_t)d, (const rafting_coutbox_t*)BUF(coutStruct), (uint32_t)rows,
+                                      (uint32_t)flags, (rafting_req_rec_t*)BUF(recsOut), (uint8_t*)BUF(tagsOut), (uint32_t)cap, &n, &unknown));
+    return (jint)n;
+}
 JNIEXPORT jint JNICALL FN(requestToInbox)(JNIEnv* env, jclass k, jobject rec, jobject entryTerms, jint row, jlong nowMs, jboolean hostResult,
                                           jobject inStruct, jint nGroups, jint entCap, jint entCount) {
     uint32_t cnt = (uint32_t)entCount;

@@ -248,8 +248,9 @@ class Engine:
 
     def step_compact(self, cin, cout, slot: int = 0, reqs=None, flags: int = 0):
         """Synchronous compact step: cin / cout are rafting_b200.compact.CompactInbox / CompactOutbox, reqs a
-        rafting_b200.compact.CompactRequests (None: rafting_step_begin_compact).  flags = abi.COMPACT_ELECTIONS carries
-        ballots, vote replies and vote requests compact (rafting_step_begin_compact_ex)."""
+        rafting_b200.compact.CompactRequests (None: rafting_step_begin_compact).  flags (rafting_step_begin_compact_ex):
+        abi.COMPACT_ELECTIONS carries ballots, vote replies and vote requests compact, abi.COMPACT_PREV_TERM AE plans whose
+        prevLogTerm lies 1..8 below the group's term; the two combine."""
         if flags:
             self.step_begin_compact_ex(slot, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags)
         elif reqs is None:

@@ -58,6 +58,8 @@ def lib():
         L.rafting_request_to_creq.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int64, C.c_int, C.POINTER(abi.CInboxC),
                                               C.c_uint32, C.POINTER(abi.CReqsC), C.c_uint32, C.c_uint32, C.c_uint32]
         L.rafting_request_to_creq_ex.argtypes = L.rafting_request_to_creq.argtypes + [C.c_uint32]
+        L.rafting_coutbox_to_requests.argtypes = [C.c_void_p, C.POINTER(abi.COutboxC), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                  C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
         L.rafting_coutbox_to_replies.argtypes = [C.POINTER(abi.COutboxC), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
                                                  C.c_void_p, C.POINTER(C.c_uint32)]
         L.rafting_outbox_apply_ranges.argtypes = [C.POINTER(abi.OutboxC), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
@@ -205,6 +207,21 @@ class Dispatch:
         if rc:
             raise ValueError(f"rafting_outbox_to_requests: rc={rc}")
         return out[:n.value], unk.value
+
+    def crequests(self, cout, rows: int, flags: int = 0, cap: int = 1 << 16):
+        """The same from a waited-for compact outbox (rafting_b200.compact.CompactOutbox) of a step begun with `flags`
+        -> (records, the tag of each record's pending entry, unknown plans); OverflowError when its escape list overflowed."""
+        out = np.zeros(cap, dtype=REQ_REC)
+        tags = np.zeros(cap, dtype=np.uint8)
+        n, unk = C.c_uint32(), C.c_uint32()
+        oc = cout.as_c()
+        rc = lib().rafting_coutbox_to_requests(self._h, C.byref(oc), rows, flags, out.ctypes.data, tags.ctypes.data, cap, C.byref(n),
+                                               C.byref(unk))
+        if rc == -5 and int(cout.counts[0]) > cout.esc_cap:                    # RAFTING_E_CAPACITY
+            raise OverflowError("escape list overflow: fetch the dense outbox (rafting_step_fetch_dense)")
+        if rc:
+            raise ValueError(f"rafting_coutbox_to_requests: rc={rc}")
+        return out[:n.value], tags[:n.value], unk.value
 
     def __del__(self):
         try:

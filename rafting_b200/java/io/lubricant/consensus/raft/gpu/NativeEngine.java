@@ -82,6 +82,7 @@ final class NativeEngine {
     static native long dispatchCreate(int nGroups, int followers, int localSlot);                // engine-to-engine peers: the dispatch loop of §4 in C
     static native void dispatchDestroy(long d);
     static native int  outboxToRequests(long d, ByteBuffer outStruct, int rows, ByteBuffer reqRecsOut, int cap);   // plans + vote broadcasts -> 64 B request records
+    static native int  coutboxToRequests(long d, ByteBuffer coutStruct, int rows, int flags, ByteBuffer reqRecsOut, ByteBuffer tagsOut, int cap);   // the same from a compact outbox, + the pending tag per record
     static native int  requestToInbox(ByteBuffer rec, ByteBuffer entryTerms, int row, long nowMs, boolean hostResult, ByteBuffer inStruct, int nGroups, int entCap, int entCount);
     static native int  outboxToReplies(ByteBuffer outStruct, int nGroups, int localSlot, ByteBuffer placed, ByteBuffer placedRow, int n, ByteBuffer replyRecsOut);
     static native void requestToCreq(ByteBuffer rec, ByteBuffer entryTerms, int row, long nowMs, boolean hostResult, ByteBuffer cinStruct, int nGroups,

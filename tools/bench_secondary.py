@@ -10,9 +10,9 @@ parity tests replay against the oracle); every step is generator kernel -> step 
 only the step kernel is inside the CUDA-event pairs (second pass over the same stream after a rollback of the tables).  Algorithmic bytes per unit are SURVEY §8(d)'s:
 B_vote = 64, B_ack(R) = 184 + 8(R-2), B_req(n) = 160 + 32 n.  Prints one JSON line per configuration.
 
---e2e instead runs config #5 end to end through the dense host path and the compact one with its request list (run_e2e);
---e2e3 [--groups G] runs config #3 end to end through the dense path, the compact path, and the compact path with
-RAFTING_COMPACT_ELECTIONS (run_e2e3)."""
+--e2e instead runs config #5 end to end through the dense host path, the compact one with its request list, and the same
+with RAFTING_COMPACT_PREV_TERM (run_e2e); --e2e3 [--groups G] runs config #3 end to end through the dense path, the compact
+path, and the compact path with RAFTING_COMPACT_ELECTIONS, without and with RAFTING_COMPACT_PREV_TERM (run_e2e3)."""
 import json
 import os
 import sys
@@ -145,13 +145,15 @@ def card():
 
 
 def run_e2e(G=524288, R=3, rows=4, settle=24, window=12, passes=3, seed=0x5EED0005):
-    """config #5 end to end through two host paths.  A window of launches is recorded on the device path; each host path then
+    """config #5 end to end through three host paths.  A window of launches is recorded on the device path; each host path then
     replays it from pinned caller-owned buffers filled before the clock starts, four launches in flight:
       dense    rafting_step_begin_host: every inbox / outbox column, the sparse ones when the step produced any
       compact  rafting_step_begin_compact_req: ev_c / op_c words, AppendEntries as 32-byte records, every other request as an
                op escape, replies in rep_c
+      prev_term  the same with RAFTING_COMPACT_PREV_TERM: AE plans whose prevLogTerm lies 1..8 below the group's term as plan_c
+               words
     Launch 0 of the window answers RPCs planned on the device path (no tags): it runs once, untimed, and the state after it
-    is where every timed pass starts.  Both paths must end in the device path's state."""
+    is where every timed pass starts.  Every path must end in the device path's state."""
     import time
     import torch
     from rafting_b200 import compact
@@ -200,52 +202,65 @@ def run_e2e(G=524288, R=3, rows=4, settle=24, window=12, passes=3, seed=0x5EED00
     cout0 = compact.CompactOutbox(rows, G, F, esc_cap=rows * G * (F + 2))
     e.step_compact(enc0, cout0, reqs=enc0.reqs if enc0.reqs is not None else compact.CompactRequests())   # launch 0, untimed
     e.checkpoint()
-    tags, sent_term, sent_inc = cout0.tags(), cout0.current_term.copy(), cout0.incarnation.copy()
+    tags0, sent_term0, sent_inc0 = cout0.tags(rpc_only=True), cout0.current_term.copy(), cout0.incarnation.copy()
     _, out_off = engine.Engine.compact_layout(rows, G, F, 0, ESC_CAP)
     keep, couts = [], []
     for sl in range(NSL):
         t = torch.zeros(int(out_off[11]), dtype=torch.uint8).pin_memory(); keep.append(t)
         couts.append(compact.outbox_in_block(t.numpy(), out_off, rows, G, F, ESC_CAP))
-    up_c, esc_in, esc_out, acks, ae, entries = [], [], [], 0, 0, 0
-    for k in range(1, window):                                            # record pass (untimed): the tags the engine hands out
-        ci = compact.encode_inbox(inboxes[k], tags, sent_term, sent_inc)
-        q = ci.reqs if ci.reqs is not None else compact.CompactRequests()
-        in_off, _ = engine.Engine.compact_layout(rows, G, F, len(ci.esc), ESC_CAP)
-        t = torch.zeros(int(in_off[5]), dtype=torch.uint8).pin_memory(); keep.append(t)
-        ci = compact.inbox_in_block(t.numpy(), in_off, ci)
-        r_off = engine.Engine.compact_req_layout(len(q.req), len(q.op_esc), len(q.ent_terms))
-        t = torch.zeros(max(1, int(r_off[3])), dtype=torch.uint8).pin_memory(); keep.append(t)
-        blk = t.numpy()
-        views = []
-        for a, off in ((q.req, r_off[0]), (q.op_esc, r_off[1]), (q.ent_terms, r_off[2])):
-            v = blk[int(off):int(off) + a.nbytes].view(a.dtype)
-            v[...] = a
-            views.append(v)
-        q = compact.CompactRequests(*views)
-        e.step_compact(ci, couts[0], reqs=q)
-        if int(couts[0].counts[0]) > ESC_CAP:
-            raise SystemExit(f"launch {k} produced {int(couts[0].counts[0])} escape records (> {ESC_CAP})")
-        tags, sent_term, sent_inc = couts[0].tags(), couts[0].current_term.copy(), couts[0].incarnation.copy()
-        cins.append(ci.as_c()); reqs.append(q.as_c())
-        span = (in_off[4] + len(ci.esc) * abi.CESC_IN.itemsize) if len(ci.esc) else (in_off[3] + ci.ev_c.nbytes)
-        up_c.append(span + (int(r_off[3]) if len(q.req) or len(q.op_esc) else 0))
-        esc_in.append((len(ci.esc), len(q.op_esc))); esc_out.append(int(couts[0].counts[0]))
-        h = inboxes[k]
+    acks = ae = entries = 0
+    for h in inboxes[1:]:
         evk = (h.ev_meta & np.uint64(0xF)).astype(np.int64)
         opk = (h.op_meta & np.uint64(0xFF)).astype(np.int64)
         acks += int(((evk == abi.EV_AE_ACK) | (evk == abi.EV_IS_ACK)).sum())
         ae += int((opk == abi.OP_AE_REQUEST).sum())
         entries += int((((h.op_meta >> np.uint64(16)) & np.uint64(0xFFFF)).astype(np.int64) * (opk == abi.OP_AE_REQUEST)).sum())
-    digest_rec = e.digest(0, G)
-    cout_c = [co.as_c() for co in couts]
     n = window - 1
+    recorded = {}
+    for path, flags in (("compact", 0), ("prev_term", abi.COMPACT_PREV_TERM)):
+        e.restore()
+        tags, sent_term, sent_inc = tags0, sent_term0, sent_inc0
+        cins, reqs, up_c, esc_in, esc_out, by_kind = [], [], [], [], [], np.zeros(4, np.int64)
+        for k in range(1, window):                                        # record pass (untimed): the tags the engine hands out
+            ci = compact.encode_inbox(inboxes[k], tags, sent_term, sent_inc)
+            q = ci.reqs if ci.reqs is not None else compact.CompactRequests()
+            in_off, _ = engine.Engine.compact_layout(rows, G, F, len(ci.esc), ESC_CAP)
+            t = torch.zeros(int(in_off[5]), dtype=torch.uint8).pin_memory(); keep.append(t)
+            ci = compact.inbox_in_block(t.numpy(), in_off, ci)
+            r_off = engine.Engine.compact_req_layout(len(q.req), len(q.op_esc), len(q.ent_terms))
+            t = torch.zeros(max(1, int(r_off[3])), dtype=torch.uint8).pin_memory(); keep.append(t)
+            blk = t.numpy()
+            views = []
+            for a, off in ((q.req, r_off[0]), (q.op_esc, r_off[1]), (q.ent_terms, r_off[2])):
+                v = blk[int(off):int(off) + a.nbytes].view(a.dtype)
+                v[...] = a
+                views.append(v)
+            q = compact.CompactRequests(*views)
+            e.step_compact(ci, couts[0], reqs=q, flags=flags)
+            if int(couts[0].counts[0]) > ESC_CAP:
+                raise SystemExit(f"{path}: launch {k} produced {int(couts[0].counts[0])} escape records (> {ESC_CAP})")
+            tags, sent_term, sent_inc = couts[0].tags(rpc_only=True), couts[0].current_term.copy(), couts[0].incarnation.copy()
+            cins.append(ci.as_c()); reqs.append(q.as_c())
+            span = (in_off[4] + len(ci.esc) * abi.CESC_IN.itemsize) if len(ci.esc) else (in_off[3] + ci.ev_c.nbytes)
+            up_c.append(span + (int(r_off[3]) if len(q.req) or len(q.op_esc) else 0))
+            esc_in.append((len(ci.esc), len(q.op_esc))); esc_out.append(int(couts[0].counts[0]))
+            by_kind += np.bincount(couts[0].esc["kind"][:int(couts[0].counts[0])].astype(np.int64), minlength=4)[:4]
+        recorded[path] = dict(cins=cins, reqs=reqs, flags=flags, exact=bool((e.digest(0, G) == digest_dev).all()),
+                              stats={"h2d_bytes_per_launch": int(np.mean(up_c)),
+                                     "d2h_bytes_per_launch": int(out_off[10] + 256 * abi.CESC_OUT.itemsize + max(0, np.mean(esc_out) - 256) * abi.CESC_OUT.itemsize),
+                                     "escape_records_in_per_launch": {"events": float(np.mean([x[0] for x in esc_in])), "ops": float(np.mean([x[1] for x in esc_in]))},
+                                     "escape_records_out_per_launch": float(np.mean(esc_out)),
+                                     "escape_records_out_per_launch_by_kind": {kd: float(by_kind[i] / n) for i, kd in ((1, "plan"), (2, "ballot"), (3, "reply"))},
+                                     "dense_fallbacks_per_launch": 0.0})
+    cout_c = [co.as_c() for co in couts]
 
-    def compact_pass():
+    def compact_pass(path):
+        rec = recorded[path]
         for j in range(n):
             sl = j % NSL
             if j >= NSL:
                 e.step_wait_compact(sl)
-            e.step_begin_compact_req(sl, cins[j], reqs[j], cout_c[sl])
+            e.step_begin_compact_ex(sl, rec["cins"][j], rec["reqs"][j], cout_c[sl], rec["flags"])
         for sl in range(NSL):
             e.step_wait_compact(sl)
 
@@ -281,7 +296,7 @@ def run_e2e(G=524288, R=3, rows=4, settle=24, window=12, passes=3, seed=0x5EED00
             e.step_wait_slot(sl)
 
     res = {}
-    for name, fn in (("dense", dense_pass), ("compact", compact_pass)):
+    for name, fn in (("dense", dense_pass), ("compact", lambda: compact_pass("compact")), ("prev_term", lambda: compact_pass("prev_term"))):
         e.restore(); fn()                                                 # untimed: every slot's staging exists before the clock
         exact = bool((e.digest(0, G) == digest_dev).all())
         t0 = time.perf_counter()
@@ -293,24 +308,26 @@ def run_e2e(G=524288, R=3, rows=4, settle=24, window=12, passes=3, seed=0x5EED00
         res[name] = {"acks_per_s": acks * passes / spent, "ae_requests_per_s": ae * passes / spent, "entries_per_s": entries * passes / spent,
                      "launches": n * passes, "exact": exact}
     res["dense"].update({"path": "rafting_step_begin_host", "h2d_bytes_per_launch": int(up_d), "d2h_bytes_per_launch": int(down_d)})
-    res["compact"].update({"path": "rafting_step_begin_compact_req", "h2d_bytes_per_launch": int(np.mean(up_c)),
-                           "d2h_bytes_per_launch": int(out_off[10] + 256 * abi.CESC_OUT.itemsize + max(0, np.mean(esc_out) - 256) * abi.CESC_OUT.itemsize),
-                           "escape_records_in_per_launch": {"events": float(np.mean([x[0] for x in esc_in])), "ops": float(np.mean([x[1] for x in esc_in]))}, "escape_records_out_per_launch": float(np.mean(esc_out))})
+    res["compact"].update({"path": "rafting_step_begin_compact_req", **recorded["compact"]["stats"], "record_pass_exact": recorded["compact"]["exact"]})
+    res["prev_term"].update({"path": "rafting_step_begin_compact_ex(RAFTING_COMPACT_PREV_TERM)", **recorded["prev_term"]["stats"],
+                             "record_pass_exact": recorded["prev_term"]["exact"]})
     rec = {"config": "config5_e2e", "groups": G, "replicas": R, "rows_per_launch": rows, "window_launches": n, "passes": passes,
            "launches_in_flight": NSL, "units_per_launch": {"acks": acks / n, "ae_requests": ae / n, "entries": entries / n},
-           "record_pass_exact": bool((digest_rec == digest_dev).all()), "card": card(), **res}
+           "card": card(), **res}
     print(json.dumps(rec), flush=True)
     return rec
 
 
 def run_e2e3(G=262144, R=5, rows=1, settle=4, window=12, passes=3, seed=0x5EED0003, local_slot=2):
-    """config #3 (vote storm, PreVote on) end to end through three host paths.  A window of launches is recorded on the device
+    """config #3 (vote storm, PreVote on) end to end through four host paths.  A window of launches is recorded on the device
     path; each host path then replays it from pinned caller-owned buffers filled before the clock starts, four launches in
     flight:
       dense      rafting_step_begin_host
       compact    rafting_step_begin_compact_req: every vote reply and ballot an escape record, every vote request an op escape
       elections  rafting_step_begin_compact_ex(RAFTING_COMPACT_ELECTIONS): replies as ev_c words, ballots as plan_c lanes,
                  vote requests as records
+      elections_prev_term   the same with RAFTING_COMPACT_PREV_TERM: AE plans whose prevLogTerm lies 1..8 below the group's
+                 term (the first heartbeats of new leaders) as plan_c words
     Both compact paths get the escape capacity --e2e uses (rows x G x F / 8 records down); a launch whose escape list overflows
     it is completed with rafting_step_fetch_dense, and those bytes are counted.  Launch 0 of the window answers ballots of the
     device path (no tags): it runs once, untimed, and the state after it is where every pass starts.  Every path must end in
@@ -318,7 +335,7 @@ def run_e2e3(G=262144, R=5, rows=1, settle=4, window=12, passes=3, seed=0x5EED00
     import time
     import torch
     from rafting_b200 import compact
-    F, NSL, EL = R - 1, 4, abi.COMPACT_ELECTIONS
+    F, NSL, EL, PT = R - 1, 4, abi.COMPACT_ELECTIONS, abi.COMPACT_PREV_TERM
     dev = torch.device("cuda:0")
     L = _bind()
     # ---- record the window on the device path ----
@@ -380,14 +397,14 @@ def run_e2e3(G=262144, R=5, rows=1, settle=4, window=12, passes=3, seed=0x5EED00
     down_cols = int(out_off[10])
     dense_down = dense_outbox()[1]
     recorded = {}
-    for path, flags in (("compact", 0), ("elections", EL)):
+    for path, flags in (("compact", 0), ("elections", EL), ("elections_prev_term", EL | PT)):
         e.restore()
         nxt = None
         if flags:
             d0 = compact.decode_outbox(cout0, elections=True)
             nxt = dict(tags=cout0.tags(rpc_only=True), sent_term=cout0.current_term.copy(), sent_inc=cout0.incarnation.copy(),
                        ballot_term=d0.ballot_term.copy(), ballot_inc=d0.ballot_meta >> np.uint64(32), ballot_tags=cout0.ballot_tags())
-        cins, reqs, up, down, esc_ev, esc_op, esc_out, fallbacks = [], [], [], [], [], [], [], 0
+        cins, reqs, up, down, esc_ev, esc_op, esc_out, fallbacks, by_kind = [], [], [], [], [], [], [], 0, np.zeros(4, np.int64)
         for k in range(1, window):
             if flags:
                 ci = compact.encode_inbox(inboxes[k], nxt["tags"], nxt["sent_term"], nxt["sent_inc"], elections=True,
@@ -415,14 +432,16 @@ def run_e2e3(G=262144, R=5, rows=1, settle=4, window=12, passes=3, seed=0x5EED00
             fallbacks += over
             down.append(down_cols + max(min(n_out, ESC_CAP), min(256, ESC_CAP)) * abi.CESC_OUT.itemsize + (dense_down if over else 0))
             esc_ev.append(len(ci.esc)); esc_op.append(len(q.op_esc)); esc_out.append(n_out)
+            by_kind += np.bincount(co.esc["kind"][:n_out].astype(np.int64), minlength=4)[:4]
             if flags:
-                d = compact.decode_outbox(co, elections=True)
+                d = compact.decode_outbox(co, elections=True, prev_term=bool(flags & PT))
                 nxt = dict(tags=co.tags(rpc_only=True), sent_term=co.current_term.copy(), sent_inc=co.incarnation.copy(),
                            ballot_term=d.ballot_term.copy(), ballot_inc=d.ballot_meta >> np.uint64(32), ballot_tags=co.ballot_tags())
         recorded[path] = dict(cins=cins, reqs=reqs, flags=flags, exact=bool((e.digest(0, G) == digest_dev).all()),
                               stats={"h2d_bytes_per_launch": int(np.mean(up)), "d2h_bytes_per_launch": int(np.mean(down)),
                                      "escape_records_in_per_launch": {"events": float(np.mean(esc_ev)), "ops": float(np.mean(esc_op))},
                                      "escape_records_out_per_launch": float(np.mean(esc_out)),
+                                     "escape_records_out_per_launch_by_kind": {kd: float(by_kind[i] / n) for i, kd in ((1, "plan"), (2, "ballot"), (3, "reply"))},
                                      "dense_fallbacks_per_launch": fallbacks / n})
     # ---- the pinned buffers of the timed passes ----
     couts, fall = [], []
@@ -468,7 +487,8 @@ def run_e2e3(G=262144, R=5, rows=1, settle=4, window=12, passes=3, seed=0x5EED00
             finish(sl)
 
     res = {}
-    for name, fn in (("dense", dense_pass), ("compact", lambda: compact_pass("compact")), ("elections", lambda: compact_pass("elections"))):
+    for name, fn in (("dense", dense_pass), ("compact", lambda: compact_pass("compact")), ("elections", lambda: compact_pass("elections")),
+                     ("elections_prev_term", lambda: compact_pass("elections_prev_term"))):
         e.restore(); fn()                                                 # untimed: every slot's staging exists before the clock
         exact = bool((e.digest(0, G) == digest_dev).all())
         rates = []
@@ -487,6 +507,8 @@ def run_e2e3(G=262144, R=5, rows=1, settle=4, window=12, passes=3, seed=0x5EED00
                            "record_pass_exact": recorded["compact"]["exact"]})
     res["elections"].update({"path": "rafting_step_begin_compact_ex(RAFTING_COMPACT_ELECTIONS)", **recorded["elections"]["stats"],
                              "record_pass_exact": recorded["elections"]["exact"]})
+    res["elections_prev_term"].update({"path": "rafting_step_begin_compact_ex(RAFTING_COMPACT_ELECTIONS | RAFTING_COMPACT_PREV_TERM)",
+                                       **recorded["elections_prev_term"]["stats"], "record_pass_exact": recorded["elections_prev_term"]["exact"]})
     rec = {"config": "config3_e2e", "groups": G, "replicas": R, "rows_per_launch": rows, "window_launches": n, "passes": passes,
            "launches_in_flight": NSL, "escape_cap_down": ESC_CAP,
            "units_per_launch": {k: v / n for k, v in units.items()}, "card": card(), **res}
