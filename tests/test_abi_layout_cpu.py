@@ -1,39 +1,19 @@
-"""Field-by-field layout check of every Python mirror (ctypes Structures in rafting_b200/abi.py, numpy record dtypes in abi.py /
-ingest.py / engine.py / durable.py) against the C headers: a probe compiled by gcc from include/*.h prints sizeof and offsetof
-for each struct and field, and the mirrors must agree.  Host only — the headers are plain C."""
-import ctypes as C
+"""Field-by-field layout check of every Python mirror (MIRRORS of tools/gen_java_layout.py: ctypes Structures in
+rafting_b200/abi.py, numpy record dtypes in abi.py / ingest.py / engine.py / durable.py / workload.py) against the C headers: a
+probe compiled by gcc from include/*.h prints sizeof and offsetof for each struct and field, and the mirrors must agree.  Host
+only — the headers are plain C."""
+import importlib.util
 import os
 import shutil
 import subprocess
 
-import numpy as np
 import pytest
 
-from rafting_b200 import abi, durable, engine, ingest, workload
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-# C struct name -> Python mirror
-MIRRORS = {
-    "rafting_cfg_t": abi.Cfg, "rafting_inbox_t": abi.InboxC, "rafting_outbox_t": abi.OutboxC, "rafting_group_init_t": abi.GroupInit,
-    "rafting_follower_state_t": abi.FollowerState, "rafting_group_state_t": abi.GroupState, "rafting_lease_t": abi.LeaseC,
-    "rafting_cinbox_t": abi.CInboxC, "rafting_coutbox_t": abi.COutboxC,
-    "rafting_cesc_in_t": abi.CESC_IN, "rafting_cesc_out_t": abi.CESC_OUT,
-    "rafting_entry_ref_t": engine.Engine.ENTRY_REF,
-    "rafting_frame_t": ingest.FRAME, "rafting_batch_rec_t": ingest.BATCH_REC, "rafting_ack_rec_t": ingest.ACK_REC,
-    "rafting_req_rec_t": ingest.REQ_REC, "rafting_apply_rec_t": ingest.APPLY_REC,
-    "rafting_stable_t": durable.Stable,
-    "rafting_wl_cfg_t": workload.WlCfg,
-}
-
-
-RENAMED = {"rafting_lease_t": {"inbox": "in", "outbox": "out"}}       # `in` is a Python keyword
-
-
-def _fields(m):
-    if isinstance(m, np.dtype):
-        return [(n, m.fields[n][1], m.fields[n][0].itemsize) for n in m.names], m.itemsize
-    return [(n, getattr(m, n).offset, getattr(m, n).size) for n, *_ in m._fields_], C.sizeof(m)
+_spec = importlib.util.spec_from_file_location("gen_java_layout", os.path.join(ROOT, "tools", "gen_java_layout.py"))
+gen = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(gen)
+MIRRORS, RENAMED, _fields = gen.MIRRORS, gen.RENAMED, gen.fields
 
 
 @pytest.mark.skipif(shutil.which("gcc") is None, reason="no gcc")
@@ -67,8 +47,4 @@ def test_every_mirror_has_the_layout_the_headers_compile_to(tmp_path):
 def test_generated_java_layout_constants_are_current():
     """rafting_b200/java/.../Layout.java (offsets the Java side uses on direct ByteBuffers) is generated from the headers by
     tools/gen_java_layout.py; a header change without regenerating it fails here."""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("gen_java_layout", os.path.join(ROOT, "tools", "gen_java_layout.py"))
-    gen = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(gen)
     assert open(gen.OUT).read() == gen.generate(), "run `python tools/gen_java_layout.py`"

@@ -1,6 +1,6 @@
 """Elections through the compact host path, on CPU (RAFTING_COMPACT_ELECTIONS): ballots as plan_c lanes, vote replies as
 ev_c words and inbound vote requests as records are lossless.  A numpy restatement of the engine's flagged unpack / pack
-kernels (tests/compact_vote_model.py) runs around the oracle on the config #3 vote storm and the config #5 mixed stream:
+kernels (tests/compact_model.py) runs around the oracle on the config #3 vote storm and the config #5 mixed stream:
 every dense inbox must survive encode -> unpack on every column the step reads, every dense outbox pack -> decode."""
 import numpy as np
 import pytest
@@ -8,88 +8,30 @@ import pytest
 from oracle import binding
 from rafting_b200 import abi, compact, workload
 from tests import compact_model as model
-from tests import compact_req_model as req_model
-from tests import compact_vote_model as vote_model
 from tests import harness
-from tests.test_compact_requests_cpu import _epoch, assert_step_reads_the_same
+from tests.compact_model import EL, assert_step_reads_the_same
 
 U64 = np.uint64
-EL = dict(elections=True)
-
-
-class Ratios:
-    """How much of a stream's election traffic travelled compact."""
-
-    def __init__(self):
-        self.replies = self.reply_words = self.ballots = self.ballot_lanes = self.vote_reqs = self.vote_records = 0
-        self.ae = self.ae_records = 0
-
-    def add(self, ib: abi.Inbox, ci: compact.CompactInbox, dense: abi.Outbox, co: compact.CompactOutbox):
-        ek = (ib.ev_meta & U64(0xF)).astype(np.int64)
-        self.replies += int(((ek == abi.EV_PV_REPLY) | (ek == abi.EV_RV_REPLY)).sum())
-        wk = (ci.ev_c & np.uint32(0xF)).astype(np.int64)
-        self.reply_words += int(((wk == abi.EV_PV_REPLY) | (wk == abi.EV_RV_REPLY)).sum())
-        self.ballots += int((dense.ballot_meta != 0).sum())
-        self.ballot_lanes += int(((co.plan_c[:, :, 0] & np.uint32(7)) >= abi.CPLAN_PREVOTE).sum())
-        ok = (ib.op_meta & U64(0xFF)).astype(np.int64)
-        self.vote_reqs += int(((ok == abi.OP_PREVOTE_REQ) | (ok == abi.OP_VOTE_REQ)).sum())
-        self.ae += int((ok == abi.OP_AE_REQUEST).sum())
-        if ci.reqs is not None:
-            vk = (ci.reqs.req["meta"] >> np.uint32(11)) & np.uint32(3)
-            self.vote_records += int((vk != 0).sum())
-            self.ae_records += int((vk == 0).sum())
-
-    def assert_mostly_compact(self, votes=True):
-        if votes:
-            assert self.replies > 500 and self.ballots > 100 and self.vote_reqs > 100, vars(self)
-            assert self.reply_words >= 0.9 * self.replies, vars(self)
-            assert self.ballot_lanes >= 0.9 * self.ballots, vars(self)
-            assert self.vote_records >= 0.9 * self.vote_reqs, vars(self)
-
-
-def _flagged_next(dense: abi.Outbox, co: compact.CompactOutbox):
-    """What a pump keeps from a flagged step for encoding the next one: the tags of the RPCs in flight, the term / incarnation
-    of its plans, and the term / incarnation of the ballots the next vote replies answer."""
-    return dict(tags=co.tags(rpc_only=True), sent_term=co.current_term.copy(), sent_inc=co.incarnation.copy(),
-                ballot_term=dense.ballot_term.copy(), ballot_inc=dense.ballot_meta >> U64(32), ballot_tags=co.ballot_tags())
-
-
-def _encode(ib, nxt):
-    if nxt is None:
-        return compact.encode_inbox(ib, None, None, None, **EL)
-    return compact.encode_inbox(ib, nxt["tags"], nxt["sent_term"], nxt["sent_inc"], ballot_term=nxt["ballot_term"],
-                                ballot_inc=nxt["ballot_inc"], ballot_tags=nxt["ballot_tags"], **EL)
-
-
-def _storm(G, R, rows, seed=0x5EED0003):
-    F = R - 1
-    cfg = abi.make_cfg(replicas=R, local_slot=1, max_groups=G, max_rows=rows, entry_pool_cap=workload.POOL_TERMS)
-    o = binding.Oracle(cfg)
-    init = harness.init_array(G, terms=1 + np.arange(G) % 5)
-    init["last_index"] = 100 + np.arange(G) % 50
-    init["last_term"] = 1 + np.arange(G) % 5
-    o.open_bulk(0, init)
-    return o, workload.make_wl(seed, rows, G, F, local_slot=1)
 
 
 @pytest.mark.parametrize("rows", [1, 2])
 def test_vote_storm_round_trips_through_the_election_words_and_mostly_travels_compact(rows):
     G, R, steps, settle = 256, 5, 16, 2
     F = R - 1
-    o, w = _storm(G, R, rows)
+    o, w = model.storm(G, R, rows)
     st = model.InFlight(G, F)
     g_term = np.array([o.export(g).current_term for g in range(G)], dtype=np.int64)
-    prev, nxt, ratios = None, None, Ratios()
+    prev, nxt, ratios = None, None, model.Ratios()
     for k in range(steps):
         ib = workload.vote_inbox_host(w, k, prev)
-        ci = _encode(ib, nxt)
-        assert_step_reads_the_same(ib, vote_model.unpack_el(ci, g_term, st), where=f"encode -> unpack, step {k}")
+        ci = model.encode(ib, nxt, EL, empty_list=False)
+        assert_step_reads_the_same(ib, model.unpack(ci, g_term, st, EL), where=f"encode -> unpack, step {k}")
         dense = o.step(ib)
-        co = vote_model.pack_el(dense, _epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G)
-        harness.assert_outbox_equal(dense, compact.decode_outbox(co, **EL), where=f"pack -> decode, step {k}")
+        co = model.pack(dense, model.oracle_epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G, flags=EL, replies=True)
+        harness.assert_outbox_equal(dense, compact.decode_outbox(co, elections=True), where=f"pack -> decode, step {k}")
         if k >= settle:
             ratios.add(ib, ci, dense, co)
-        prev, nxt, g_term = dense, _flagged_next(dense, co), dense.current_term.copy()
+        prev, nxt, g_term = dense, model.next_of(dense, co), dense.current_term.copy()
     if rows == 1:
         ratios.assert_mostly_compact()
     else:
@@ -109,33 +51,33 @@ def test_mixed_stream_round_trips_with_the_flag_and_its_appendentries_stay_as_co
     w = workload.make_wl(0x5EED0005, rows, G, F)
     st, st0 = model.InFlight(G, F), model.InFlight(G, F)
     g_term = np.array([o.export(g).current_term for g in range(G)], dtype=np.int64)
-    prev, nxt, prev0 = None, None, (None, None, None)
-    flagged, plain = Ratios(), Ratios()
+    prev, nxt, nxt0 = None, None, None
+    flagged, plain = model.Ratios(), model.Ratios()
     for k in range(steps):
         ib = workload.mixed_inbox_host(w, k, prev)
-        ci = _encode(ib, nxt)
-        ci0 = compact.encode_inbox(ib, *prev0)                                  # the same step without the flag
-        assert_step_reads_the_same(ib, vote_model.unpack_el(ci, g_term, st), where=f"encode -> unpack, step {k}")
+        ci = model.encode(ib, nxt, EL, empty_list=False)
+        ci0 = model.encode(ib, nxt0, 0, empty_list=False)                      # the same step without the flag
+        assert_step_reads_the_same(ib, model.unpack(ci, g_term, st, EL), where=f"encode -> unpack, step {k}")
         dense = o.step(ib)
-        co = vote_model.pack_el(dense, _epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G)
-        harness.assert_outbox_equal(dense, compact.decode_outbox(co, **EL), where=f"pack -> decode, step {k}")
-        req_model.unpack_req(ci0, g_term, st0)
-        co0 = req_model.pack_req(dense, _epoch(o, G), st0, esc_cap=rows * G * F + 2 * rows * G)
+        co = model.pack(dense, model.oracle_epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G, flags=EL, replies=True)
+        harness.assert_outbox_equal(dense, compact.decode_outbox(co, elections=True), where=f"pack -> decode, step {k}")
+        model.unpack(ci0, g_term, st0)
+        co0 = model.pack(dense, model.oracle_epoch(o, G), st0, esc_cap=rows * G * F + 2 * rows * G, replies=True)
         if k >= settle:
             flagged.add(ib, ci, dense, co)
             plain.add(ib, ci0, dense, co0)
-        prev, nxt, g_term = dense, _flagged_next(dense, co), dense.current_term.copy()
-        prev0 = (co0.tags(), co0.current_term.copy(), co0.incarnation.copy())
+        prev, nxt, g_term = dense, model.next_of(dense, co), dense.current_term.copy()
+        nxt0 = model.next_of(dense, co0)
     assert flagged.ae > 1000 and flagged.ae_records == plain.ae_records, (vars(flagged), vars(plain))
     assert flagged.ballots > 0 and flagged.ballot_lanes > 0, vars(flagged)         # four rows: many ballots are superseded
 
 
 def _one_step(o, ib, nxt, st, G, esc_cap=4096):
-    ci = _encode(ib, nxt)
-    assert_step_reads_the_same(ib, vote_model.unpack_el(ci, np.array([o.export(g).current_term for g in range(G)]), st))
+    ci = model.encode(ib, nxt, EL, empty_list=False)
+    assert_step_reads_the_same(ib, model.unpack(ci, np.array([o.export(g).current_term for g in range(G)]), st, EL))
     dense = o.step(ib)
-    co = vote_model.pack_el(dense, _epoch(o, G), st, esc_cap=esc_cap)
-    harness.assert_outbox_equal(dense, compact.decode_outbox(co, **EL))
+    co = model.pack(dense, model.oracle_epoch(o, G), st, esc_cap=esc_cap, flags=EL, replies=True)
+    harness.assert_outbox_equal(dense, compact.decode_outbox(co, elections=True))
     return ci, dense, co
 
 
@@ -160,7 +102,7 @@ def test_every_rule_a_vote_breaks_sends_it_in_full():
     esc = co.esc[:int(co.counts[0])]
     assert [(int(r["kind"]), int(r["slot"])) for r in esc if r["kind"] == abi.CESC_BALLOT] == [(abi.CESC_BALLOT, 1)]
     assert ci.reqs is not None and ci.reqs.req["slot"].tolist() == [G + 1] and len(ci.reqs.op_esc) == 0
-    nxt = _flagged_next(dense, co)
+    nxt = model.next_of(dense, co)
     # step 2: the replies, one rule broken per group
     ib = abi.Inbox(rows, G, F)
     inc = dense.ballot_meta[0] >> U64(32)
@@ -206,23 +148,23 @@ def test_a_ballot_next_to_a_plan_is_escaped_and_a_malformed_vote_record_is_answe
     dense.plan_meta[0, 4, 1] = abi.PLAN_AE | (int(dense.incarnation[4]) << 32)               # one that takes a tag
     dense.plan_epoch[0, 4, 1] = 7; dense.plan_lc[0, 4, 1] = (20, 0); dense.plan_pp[0, 4, 1] = (20, 3)
     st = model.InFlight(G, F)
-    co = vote_model.pack_el(dense, _epoch(o, G), st, esc_cap=64)
+    co = model.pack(dense, model.oracle_epoch(o, G), st, esc_cap=64, flags=EL, replies=True)
     kinds = co.plan_c[0, :, :] & np.uint32(7)
     assert (kinds[3] != abi.CPLAN_PREVOTE).all() and (kinds[4] != abi.CPLAN_PREVOTE).all()
     assert (np.delete(kinds, [3, 4], axis=0) == abi.CPLAN_PREVOTE).all()
     assert sorted(int(r["slot"]) for r in co.esc[:int(co.counts[0])] if r["kind"] == abi.CESC_BALLOT) == [3, 4]
     assert int(st.bits[3].sum()) == 0 and int(st.bits[4].sum()) == 1 and int(co.counts[1]) == G
-    harness.assert_outbox_equal(dense, compact.decode_outbox(co, **EL), where="ballot next to a plan")
+    harness.assert_outbox_equal(dense, compact.decode_outbox(co, elections=True), where="ballot next to a plan")
     # a vote reply on the AE plan's lane answers the escaped ballot, not the plan: it travels in full, its escaped word names
     # no tag, and the plan's tag stays taken
-    nxt = _flagged_next(dense, co)
+    nxt = model.next_of(dense, co)
     assert nxt["tags"][0, 4, 1] < 32 and nxt["ballot_tags"][0, 4, 1] == abi.CTAG_NONE
     ib = abi.Inbox(rows, G, F)
     for f in range(F):
         ib.vote_reply(0, 4, f, harness.T0 + 20, int(dense.ballot_meta[0, 4]) >> 32, 3, False, pre=True)
-    ci = _encode(ib, nxt)
+    ci = model.encode(ib, nxt, EL, empty_list=False)
     assert (ci.ev_c[0, 4] == (abi.CEV_ESCAPED | (abi.CTAG_NONE << 8))).all() and len(ci.esc) == F
-    vote_model.unpack_el(ci, np.full(G, 3, np.int64), st)
+    model.unpack(ci, np.full(G, 3, np.int64), st, EL)
     assert int(st.bits[4, 1]) == 1 << int(nxt["tags"][0, 4, 1])
     # vote records the engine must refuse: a count, a d_commit, kind 3; and a vote record in an unflagged step
     ci = compact.CompactInbox(rows, G, F)
@@ -234,15 +176,15 @@ def test_a_ballot_next_to_a_plan_is_escaped_and_a_malformed_vote_record_is_answe
     req["d_commit"] = [0, 5, 0, 0]
     req["term"], req["prev_index"] = 5, 20
     ci.reqs = compact.CompactRequests(req)
-    ib = vote_model.unpack_el(ci, np.full(G, 3, np.int64), model.InFlight(G, F))
+    ib = model.unpack(ci, np.full(G, 3, np.int64), model.InFlight(G, F), EL)
     assert [int(ib.op_meta[0, g]) & 0xFF for g in range(4)] == [abi.COP_MALFORMED] * 3 + [abi.OP_PREVOTE_REQ]
-    ib0 = req_model.unpack_req(ci, np.full(G, 3, np.int64), model.InFlight(G, F))
+    ib0 = model.unpack(ci, np.full(G, 3, np.int64), model.InFlight(G, F))
     assert [int(ib0.op_meta[0, g]) & 0xFF for g in range(4)] == [abi.COP_MALFORMED] * 4
 
 
 def test_without_the_flag_the_codec_is_unchanged():
     G, R, rows, steps = 64, 5, 2, 6
-    o, w = _storm(G, R, rows)
+    o, w = model.storm(G, R, rows)
     prev = None
     for k in range(steps):
         ib = workload.vote_inbox_host(w, k, prev)
@@ -266,7 +208,7 @@ def test_native_election_writers_match_the_encoder_directly_and_through_the_jni_
     from tests import jni_exec
     G, R, rows, steps = 128, 5, 1, 8
     F = R - 1
-    o, w = _storm(G, R, rows)
+    o, w = model.storm(G, R, rows)
     st = model.InFlight(G, F)
     pend = ingest.Pending()
     prev, nxt, seq_of, next_seq = None, None, {}, [1] * F
@@ -285,7 +227,7 @@ def test_native_election_writers_match_the_encoder_directly_and_through_the_jni_
 
     for k in range(steps):
         ib = workload.vote_inbox_host(w, k, prev)
-        want = _encode(ib, nxt)
+        want = model.encode(ib, nxt, EL, empty_list=False)
         got = compact.CompactInbox(rows, G, F)
         got.row_base[:] = want.row_base
         got.op_c[:] = want.op_c
@@ -321,10 +263,10 @@ def test_native_election_writers_match_the_encoder_directly_and_through_the_jni_
             records += len(p.req)
         words += int(((want.ev_c & np.uint32(0xF)) == abi.EV_PV_REPLY).sum() + ((want.ev_c & np.uint32(0xF)) == abi.EV_RV_REPLY).sum())
         escaped += n_esc
-        vote_model.unpack_el(want, np.zeros(G, np.int64), st)                    # frees the tags the replies answer
+        model.unpack(want, np.zeros(G, np.int64), st, EL)                    # frees the tags the replies answer
         dense = o.step(ib)
-        co = vote_model.pack_el(dense, _epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G)
-        prev, nxt = dense, _flagged_next(dense, co)
+        co = model.pack(dense, model.oracle_epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G, flags=EL, replies=True)
+        prev, nxt = dense, model.next_of(dense, co)
         seq_of = {}
         for r, g in np.argwhere(dense.ballot_meta != 0):                        # the ballot leaves on every lane
             r, g = int(r), int(g)

@@ -1,5 +1,5 @@
 """AE plans with an older prevLogTerm through the compact host path, on CPU (RAFTING_COMPACT_PREV_TERM): a numpy restatement of
-the flagged pack_kernel (tests/compact_prev_term_model.py) runs around the oracle on the config #3 vote storm and the config #5
+the flagged pack_kernel (tests/compact_model.py) runs around the oracle on the config #3 vote storm and the config #5
 mixed stream with flags 4 and 5.  Every dense outbox must survive pack -> decode, every dense inbox (acks to kind-7 plans
 included) encode -> unpack.  rafting_coutbox_to_requests must emit what rafting_outbox_to_requests emits for the decoded
 outbox, for every flags value a step may carry."""
@@ -11,38 +11,10 @@ import pytest
 from oracle import binding
 from rafting_b200 import abi, compact, ingest, workload
 from tests import compact_model as model
-from tests import compact_prev_term_model as pt_model
 from tests import harness
-from tests.test_compact_elections_cpu import _flagged_next, _storm
-from tests.test_compact_requests_cpu import _epoch, assert_step_reads_the_same
+from tests.compact_model import EL, PT
 
 U64 = np.uint64
-EL, PT = abi.COMPACT_ELECTIONS, abi.COMPACT_PREV_TERM
-
-
-def next_of(dense: abi.Outbox, co: compact.CompactOutbox, flags: int) -> dict:
-    """What a pump keeps from a step begun with `flags` for encoding the next one, whatever flags that one carries: the tags
-    of the RPCs in flight (kind-7 plans included), the term / incarnation of its plans, and the ballots' (compact ones only
-    under RAFTING_COMPACT_ELECTIONS)."""
-    if flags & EL:
-        return _flagged_next(dense, co)
-    rows, G, F = co.rows, co.n, co.F
-    return dict(tags=co.tags(rpc_only=True), sent_term=co.current_term.copy(), sent_inc=co.incarnation.copy(),
-                ballot_term=np.zeros((rows, G), np.int64), ballot_inc=np.zeros((rows, G), U64),
-                ballot_tags=np.full((rows, G, F), abi.CTAG_NONE, np.uint8))
-
-
-def encode(ib: abi.Inbox, nxt: dict | None, flags: int) -> compact.CompactInbox:
-    """The compact inbox of a step begun with `flags`; its request list is never None (replies then travel in rep_c)."""
-    el = bool(flags & EL)
-    if nxt is None:
-        ci = compact.encode_inbox(ib, None, None, None, elections=el)
-    else:
-        ci = compact.encode_inbox(ib, nxt["tags"], nxt["sent_term"], nxt["sent_inc"], elections=el, ballot_term=nxt["ballot_term"],
-                                  ballot_inc=nxt["ballot_inc"], ballot_tags=nxt["ballot_tags"])
-    if ci.reqs is None:
-        ci.reqs = compact.CompactRequests()
-    return ci
 
 
 class Pump:
@@ -55,13 +27,13 @@ class Pump:
         self.nxt = None
 
     def step(self, o, ib, g_term, where):
-        ci = encode(ib, self.nxt, self.flags)
-        assert_step_reads_the_same(ib, pt_model.unpack_pt(ci, g_term, self.st, self.flags), where=f"encode -> unpack, {where}")
+        ci = model.encode(ib, self.nxt, self.flags, empty_list=True)
+        model.assert_step_reads_the_same(ib, model.unpack(ci, g_term, self.st, self.flags), where=f"encode -> unpack, {where}")
         dense = o.step(ib)
-        co = pt_model.pack_pt(dense, _epoch(o, self.G), self.st, esc_cap=1 << 20, flags=self.flags)
+        co = model.pack(dense, model.oracle_epoch(o, self.G), self.st, esc_cap=1 << 20, flags=self.flags, replies=True)
         harness.assert_outbox_equal(dense, compact.decode_outbox(co, elections=bool(self.flags & EL), prev_term=bool(self.flags & PT)),
                                     where=f"pack -> decode, {where}")
-        self.nxt = next_of(dense, co, self.flags)
+        self.nxt = model.next_of(dense, co)
         return ci, dense, co
 
 
@@ -108,9 +80,9 @@ def _unflagged_twin(co, flags):
 def test_vote_storm_round_trips_and_new_leaders_heartbeats_travel_as_words(rows, flags):
     G, R, steps, settle = 512, 5, 16, 2
     F = R - 1
-    o, w = _storm(G, R, rows)
+    o, w = model.storm(G, R, rows)
     flagged, plain = Pump(G, F, flags), Pump(G, F, flags & EL)
-    o0, _ = _storm(G, R, rows)
+    o0, _ = model.storm(G, R, rows)
     g_term = np.array([o.export(g).current_term for g in range(G)], dtype=np.int64)
     cnt, cnt0 = Counts(G, F), Counts(G, F)
     prev = None
@@ -166,7 +138,7 @@ def _rules_case():
     o.open_bulk(0, harness.init_array(G, terms=3, last_index=400, last_term=3, commit_index=300))
     harness.elect_all(o, workload.make_wl(0x5EED0005, 1, G, F))
     dense = o.step(abi.Inbox(rows, G, F))
-    ep = _epoch(o, G)
+    ep = model.oracle_epoch(o, G)
     for name in ("plan_meta", "plan_pp", "plan_lc", "plan_epoch"):
         getattr(dense, name)[...] = 0
     term, last, commit, inc = dense.current_term, dense.last_entry["x"], dense.commit_index, dense.incarnation
@@ -190,7 +162,7 @@ def test_every_rule_a_plan_breaks_sends_it_in_full():
     dense, ep, G, F = _rules_case()
     for flags in (PT, EL | PT):
         st = model.InFlight(G, F)
-        co = pt_model.pack_pt(dense, ep, st, esc_cap=64, flags=flags)
+        co = model.pack(dense, ep, st, esc_cap=64, flags=flags, replies=True)
         k = (co.plan_c[0, :, 1] & np.uint32(7)).tolist()
         escaped = ((co.plan_c[0, :, 1] >> np.uint32(4)) & np.uint32(1)).tolist()
         seven, one = abi.CPLAN_AE_PREV_TERM, abi.PLAN_AE
@@ -205,9 +177,9 @@ def test_every_rule_a_plan_breaks_sends_it_in_full():
         # every plan took a tag, kind 7 and escaped ones alike
         assert (co.tags(rpc_only=True)[0, :14, 1] < 32).all() and (st.bits[:14, 1] == 1).all()
         harness.assert_outbox_equal(dense, compact.decode_outbox(co, elections=bool(flags & EL), prev_term=True), where=f"flags {flags}")
-        # without the flag the same outbox never holds kind 7, and its words are those of the models without the flag
+        # without the flag the same outbox never holds kind 7, and its words are those of the model without the flag
         st0 = model.InFlight(G, F)
-        co0 = pt_model.pack_pt(dense, ep, st0, esc_cap=64, flags=flags & EL)
+        co0 = model.pack(dense, ep, st0, esc_cap=64, flags=flags & EL, replies=True)
         assert not ((co0.plan_c & np.uint32(7)) == seven).any()
         assert np.array_equal(_unflagged_twin(co, flags), co0.plan_c)
 
@@ -244,7 +216,7 @@ def test_coutbox_to_requests_matches_the_dense_dispatch_on_both_streams(flags):
     # config #3 storm, one row
     G, R, rows = 256, 5, 1
     F = R - 1
-    o, w = _storm(G, R, rows)
+    o, w = model.storm(G, R, rows)
     p = Pump(G, F, flags)
     dd, dc = _dispatch_pair(G, F, 1)
     g_term = np.array([o.export(g).current_term for g in range(G)], dtype=np.int64)
@@ -277,7 +249,7 @@ def test_coutbox_to_requests_matches_the_dense_dispatch_on_both_streams(flags):
 
 def test_coutbox_to_requests_refuses_overflow_and_unknown_flags_and_the_writers_take_bit_4(tmp_path):
     dense, ep, G, F = _rules_case()
-    co = pt_model.pack_pt(dense, ep, model.InFlight(G, F), esc_cap=64, flags=PT)
+    co = model.pack(dense, ep, model.InFlight(G, F), esc_cap=64, flags=PT, replies=True)
     d = ingest.Dispatch(G, F, 0)
     recs, tags, unknown = d.crequests(co, 1, PT)
     assert len(recs) == 13 and unknown == 1 and tags.tolist() == [0] * 13     # group 8's plan names an unseen incarnation
@@ -325,7 +297,7 @@ def test_coutbox_to_requests_through_the_jni_glue(tmp_path):
         pytest.skip("no gcc")
     from tests.jni_exec import Buf, buf_of_array, buf_of_struct, fn
     dense, ep, G, F = _rules_case()
-    co = pt_model.pack_pt(dense, ep, model.InFlight(G, F), esc_cap=64, flags=EL | PT)
+    co = model.pack(dense, ep, model.InFlight(G, F), esc_cap=64, flags=EL | PT, replies=True)
     want, want_tags, _ = ingest.Dispatch(G, F, 0).crequests(co, 1, EL | PT)
     d = ingest.Dispatch(G, F, 0)
     recs, tags = np.zeros(64, dtype=ingest.REQ_REC), np.zeros(64, np.uint8)

@@ -1,10 +1,8 @@
 """Inbound requests through the compact host path, on CPU: the request list (rafting_creqs_t) and the compact replies in
-rep_c are lossless.  A numpy restatement of the engine's unpack / pack kernels (tests/compact_req_model.py) runs around the
+rep_c are lossless.  The numpy restatement of the engine's unpack / pack kernels (tests/compact_model.py) runs around the
 oracle on the config #5 mixed stream (leader churn, AppendEntries to followers, InstallSnapshot catch-up, flushes, elections):
 every dense inbox must survive encode -> unpack on every column the step reads, every dense outbox pack -> decode."""
 import ctypes as C
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -12,73 +10,10 @@ import pytest
 from oracle import binding
 from rafting_b200 import abi, compact, workload
 from tests import compact_model as model
-from tests import compact_req_model as req_model
 from tests import harness
-from tests.test_abi_layout_cpu import ROOT, _fields
 
 U64 = np.uint64
 E_INVAL = -1
-
-# C struct name -> Python mirror, for the layout probe below and tools/gen_java_layout.py
-MIRRORS = {"rafting_creq_t": abi.CREQ, "rafting_cesc_op_t": abi.CESC_OP, "rafting_creqs_t": abi.CReqsC}
-
-
-@pytest.mark.skipif(shutil.which("gcc") is None, reason="no gcc")
-def test_request_list_mirrors_have_the_layout_the_header_compiles_to(tmp_path):
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "rafting_b200.h"', 'int main(void) {']
-    for cname, m in MIRRORS.items():
-        lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
-        for n, _, _ in _fields(m)[0]:
-            lines.append(f'  printf("{cname}.{n} %zu %zu\\n", offsetof({cname}, {n}), sizeof((({cname}*)0)->{n}));')
-    lines += ['  return 0;', '}']
-    (tmp_path / "probe.c").write_text("\n".join(lines))
-    res = subprocess.run(["gcc", "-std=c11", "-I", f"{ROOT}/include", str(tmp_path / "probe.c"), "-o", str(tmp_path / "probe")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-3000:]
-    got = {}
-    for ln in subprocess.run([str(tmp_path / "probe")], capture_output=True, text=True, check=True).stdout.splitlines():
-        k, *v = ln.split()
-        got[k] = tuple(int(x) for x in v)
-    for cname, m in MIRRORS.items():
-        fields, size = _fields(m)
-        assert got[cname] == (size,), cname
-        for n, off, sz in fields:
-            assert got[f"{cname}.{n}"] == (off, sz), f"{cname}.{n}"
-
-
-def assert_step_reads_the_same(a: abi.Inbox, b: abi.Inbox, where=""):
-    """Every inbox column the step reads: lane events where present, and per group op what its kind uses (SUBMIT / TIMEOUT:
-    time, draw and unavailable mask; requests: every field, entry terms by value)."""
-    ek = (a.ev_meta & U64(0xF)) != 0
-    assert np.array_equal(a.ev_meta, b.ev_meta), where
-    for name in ("ev_tn", "ev_el"):
-        assert np.array_equal(getattr(a, name)[ek], getattr(b, name)[ek]), f"{name} {where}"
-    lo = lambda m: m & U64(0xFFFFFFFF)
-    assert np.array_equal(lo(a.op_meta), lo(b.op_meta)), f"op kind / peer / count {where}"
-    kind = (a.op_meta & U64(0xFF)).astype(np.int64)
-    has = kind != 0
-    assert np.array_equal(a.op_nr[has], b.op_nr[has]), f"op_nr {where}"
-    simple = (kind == abi.OP_SUBMIT) | (kind == abi.OP_TIMEOUT)
-    ua = a.op_ab["x"] if a.op_ab is not None else np.zeros(kind.shape, np.int64)
-    ub = b.op_ab["x"] if b.op_ab is not None else np.zeros(kind.shape, np.int64)
-    assert np.array_equal(ua[simple], ub[simple]), f"unavailable mask {where}"
-    req = has & ~simple
-    if req.any():
-        assert np.array_equal(a.op_ab[req], b.op_ab[req]) and np.array_equal(a.op_cd[req], b.op_cd[req]), f"op_ab / op_cd {where}"
-        assert np.array_equal(a.op_e[req], b.op_e[req]), f"op_e {where}"
-        for r, i in np.argwhere(kind == abi.OP_AE_REQUEST):
-            cnt = int(a.op_meta[r, i] >> U64(16)) & 0xFFFF
-            oa, ob = int(a.op_meta[r, i] >> U64(32)), int(b.op_meta[r, i] >> U64(32))
-            assert np.array_equal(a.ent_terms[oa:oa + cnt], b.ent_terms[ob:ob + cnt]), f"entry terms at {(r, i)} {where}"
-            assert ob + cnt <= b.ent_count
-
-
-def _epoch(o, G):
-    ep = np.zeros(G, dtype=abi.I64X2)
-    for g in range(G):
-        s = o.export(g)
-        ep[g] = (s.epoch_index, s.epoch_term)
-    return ep
 
 
 def test_mixed_stream_round_trips_through_the_request_list_and_mostly_travels_compact():
@@ -91,15 +26,15 @@ def test_mixed_stream_round_trips_through_the_request_list_and_mostly_travels_co
     w = workload.make_wl(0x5EED0005, rows, G, F)
     st = model.InFlight(G, F)
     g_term = np.array([o.export(g).current_term for g in range(G)], dtype=np.int64)
-    prev, tags, sent_term, sent_inc = None, None, None, None
+    prev, nxt = None, None
     ae = records = valid = compact_replies = 0
     kinds = set()
     for k in range(steps):
         ib = workload.mixed_inbox_host(w, k, prev)
-        ci = compact.encode_inbox(ib, tags, sent_term, sent_inc)
-        assert_step_reads_the_same(ib, req_model.unpack_req(ci, g_term, st), where=f"encode -> unpack, step {k}")
+        ci = model.encode(ib, nxt, 0, empty_list=False)
+        model.assert_step_reads_the_same(ib, model.unpack(ci, g_term, st), where=f"encode -> unpack, step {k}")
         dense = o.step(ib)
-        co = req_model.pack_req(dense, _epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G)
+        co = model.pack(dense, model.oracle_epoch(o, G), st, esc_cap=rows * G * F + 2 * rows * G, replies=True)
         harness.assert_outbox_equal(dense, compact.decode_outbox(co), where=f"pack -> decode, step {k}")
         kinds |= set((ib.op_meta & U64(0xFF)).ravel().tolist())
         if k >= settle:
@@ -107,7 +42,7 @@ def test_mixed_stream_round_trips_through_the_request_list_and_mostly_travels_co
             records += 0 if ci.reqs is None else len(ci.reqs.req)
             valid += int((dense.rep_meta & 1).sum())
             compact_replies += int((co.rep_c >> 7).sum())
-        prev, tags, sent_term, sent_inc = dense, co.tags(), co.current_term.copy(), co.incarnation.copy()
+        prev, nxt = dense, model.next_of(dense, co)
         g_term = dense.current_term.copy()
     assert {abi.OP_AE_REQUEST, abi.OP_FLUSH, abi.OP_SUBMIT, abi.OP_TIMEOUT} <= kinds
     assert ae > 1000 and valid > 1000, (ae, valid)
@@ -144,9 +79,9 @@ def test_every_rule_a_request_breaks_sends_it_in_full():
     assert ci.reqs.req_entries == 2 and len(ci.reqs.ent_terms) == 2 + 5 + 64            # the escapes' terms
     assert int(ci.op_c[0, 12]) & 0xF == abi.OP_SUBMIT and not (ci.op_c[0, :12] & 0xF).any()
     st = model.InFlight(G, F)
-    assert_step_reads_the_same(ib, req_model.unpack_req(ci, np.full(G, 3, np.int64), st), where="forced escapes")
+    model.assert_step_reads_the_same(ib, model.unpack(ci, np.full(G, 3, np.int64), st), where="forced escapes")
     dense = o.step(ib)
-    co = req_model.pack_req(dense, _epoch(o, G), st, esc_cap=256)
+    co = model.pack(dense, model.oracle_epoch(o, G), st, esc_cap=256, replies=True)
     harness.assert_outbox_equal(dense, compact.decode_outbox(co), where="forced escapes")
     assert (dense.rep_meta & 1).sum() >= 10
 
@@ -158,7 +93,7 @@ def test_a_step_without_requests_encodes_as_before():
     ci = compact.encode_inbox(ib, None, None, None)
     assert ci.reqs is None
     st = model.InFlight(G, R - 1)
-    back = req_model.unpack_req(ci, np.zeros(G, np.int64), st)
+    back = model.unpack(ci, np.zeros(G, np.int64), st)
     assert back.flags == abi.INBOX_NO_REQUESTS and back.op_cd is None
 
 
@@ -205,7 +140,7 @@ def test_native_placement_and_replies_match_the_encoder_and_the_dense_helpers(tm
         assert np.array_equal(got.ent_terms, want.ent_terms) and got.req_entries == want.req_entries
         escaped += len(got.op_esc)
         out = b.step(dense)
-        co = req_model.pack_req(out, _epoch(b, G), st, esc_cap=rows * G * 2)
+        co = model.pack(out, model.oracle_epoch(b, G), st, esc_cap=rows * G * 2, replies=True)
         prow = recs["row"].astype(np.uint8)
         rd = ingest.outbox_to_replies(out, G, 1, recs, prow)
         rc = ingest.coutbox_to_replies(co, G, 1, recs, prow)

@@ -9,27 +9,17 @@ import pytest
 from oracle import binding
 from rafting_b200 import abi, compact, workload
 from tests import harness
+from tests.compact_model import Driver
 
 pytestmark = pytest.mark.gpu
 U64 = np.uint64
 SEED = 0x5EED0005
 
 
-def _pair(G, R, rows, pool=None):
-    from rafting_b200 import engine
-    cfg = abi.make_cfg(replicas=R, max_groups=G, max_rows=rows, entry_pool_cap=rows * G * 50 if pool is None else pool)
-    e, o = engine.Engine(cfg), binding.Oracle(cfg)
-    init = harness.init_array(G, terms=np.arange(G) % 7)
-    e.open_bulk(0, init), o.open_bulk(0, init)
-    w1 = workload.make_wl(SEED, 1, G, R - 1)
-    harness.assert_outbox_equal(harness.elect_all(o, w1), harness.elect_all(e, w1), where="election (dense path)")
-    return e, o
-
-
 def _run_mixed(G, R, rows, steps, settle=8):
-    e, o = _pair(G, R, rows)
+    d = Driver(G, R, rows, storm=False)
+    e, o, w = d.e, d.o, d.w
     F = R - 1
-    w = workload.make_wl(SEED, rows, G, F)
     prev, tags, sent_term, sent_inc = None, None, None, None
     ae = records = valid = compact_replies = 0
     for k in range(steps):
@@ -70,8 +60,8 @@ def test_malformed_request_lists_are_answered_per_op_like_the_dense_step():
     from rafting_b200 import engine
     G, R, rows = 1024, 3, 4
     F = R - 1
-    e, o = _pair(G, R, rows)
-    w = workload.make_wl(SEED, rows, G, F)
+    d = Driver(G, R, rows, storm=False)
+    e, o, w = d.e, d.o, d.w
     prev = None
     for k in range(10):                                           # dense steps until followers receive entries
         ib = workload.mixed_inbox_host(w, k, prev)
@@ -117,8 +107,8 @@ def test_malformed_request_lists_are_answered_per_op_like_the_dense_step():
 def test_escape_overflow_with_requests_falls_back_to_the_dense_outbox():
     G, R, rows = 1024, 3, 4
     F = R - 1
-    e, o = _pair(G, R, rows)
-    w = workload.make_wl(SEED, rows, G, F)
+    d = Driver(G, R, rows, storm=False)
+    e, o, w = d.e, d.o, d.w
     ib = workload.mixed_inbox_host(w, 0, None)
     prev = o.step(ib)
     harness.assert_outbox_equal(prev, e.step(ib), where="dense step 0")
