@@ -414,9 +414,10 @@ int rafting_step_wait_slot (rafting_engine_t* e, uint32_t slot);
  *   * the (epochAtSend, lastIndexAtSend) echo stays in an HBM in-flight table: pack gives every AE / IS plan a TAG (a free
  *     slot 0..31 of its (group, follower) lane), the reply echoes the tag, unpack looks the pair up and frees the slot.
  *     No free slot (more than 32 RPCs of one lane outstanding): tag 255, and the reply must come back as an escape record.
- *   * dense steps only (no active list).  op_c carries SUBMIT / TIMEOUT ops, ev_c AE / IS acks; vote replies and anything
- *     irregular use the escape lists (vote replies, ballots and vote requests travel compact under RAFTING_COMPACT_ELECTIONS,
- *     below).  Inbound requests ride beside the inbox in a request list (rafting_creqs_t, below):
+ *   * whole-shard steps (every column sized by max_groups), or steps over an active list through
+ *     rafting_step_begin_compact_active (every column sized by n_active, below).  op_c carries SUBMIT / TIMEOUT ops, ev_c
+ *     AE / IS acks; vote replies and anything irregular use the escape lists (vote replies, ballots and vote requests travel
+ *     compact under RAFTING_COMPACT_ELECTIONS, below).  Inbound requests ride beside the inbox in a request list (rafting_creqs_t, below):
  *     AppendEntries as 32-byte records, every other request kind as an op escape.  A step without requests runs as
  *     RAFTING_INBOX_NO_REQUESTS.
  *   * wire words are 32 bits: 4 B per lane slot + 4 B per group row up, 4 B per lane slot + 1 B per group row down.
@@ -606,6 +607,25 @@ int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot /* 0..3 */
 #define RAFTING_CPLAN_DCOMMIT7(w) (((uint32_t)(w) >> 28) & 15u)           /* the dcommit of a kind-7 word */
 int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot /* 0..3 */, const rafting_cinbox_t* in_host,
                                   const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host, uint32_t flags);
+/* ACTIVE LISTS on the compact path.  A node hosts 64 K - 1 M groups and most of them are idle in any one tick; a step over
+ * the n_active busy groups gids[0 .. n_active) moves columns of n_active entries instead of max_groups.  flags and reqs mean
+ * what they mean for rafting_step_begin_compact_ex (flags 0, 1, 4 or 5; reqs == NULL: no request list).
+ *   * position i stands for gids[i].  Every wire column is sized by n = n_active in place of max_groups: op_c and op_unavail
+ *     [rows][n], ev_c and plan_c [rows][n][F], rep_c [rows][n], and the group columns commit_index ... epoch [n] by position
+ *     (the RAFTING_INBOX_COMPACT_GROUPS shape).  Every slot is positional too: row * n + i in the request list and in
+ *     ballot / reply escape records, (row * n + i) * F + f in lane escape records, both ways.  rafting_compact_layout(rows,
+ *     n_active, F, ...) and rafting_compact_req_layout give the block offsets.  gids travels in a copy of its own (pin it,
+ *     and keep it until the wait, for overlap).
+ *   * gids must be strictly increasing, every id < max_groups, 1 <= n_active <= max_groups; anything else is refused
+ *     (RAFTING_E_INVAL, RAFTING_E_CAPACITY for n_active > max_groups) before anything is enqueued, and the slot stays free.
+ *   * the in-flight table stays indexed by gid: a plan packed at position i of one step is found by its ack at whatever
+ *     position its gid holds in a later step's list, or in a whole-shard step.  Active and whole-shard compact steps, dense
+ *     steps and leased steps mix slot by slot.  Groups not in the list are untouched.
+ *   * rafting_step_wait_compact serves the step; after it, rafting_step_fetch_dense returns the dense outbox in the
+ *     COMPACT_GROUPS shape: row columns [rows][n], group columns [n] by position. */
+int rafting_step_begin_compact_active(rafting_engine_t* e, uint32_t slot /* 0..3 */, uint32_t n_active, const uint32_t* gids /* host */,
+                                      const rafting_cinbox_t* in_host, const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host,
+                                      uint32_t flags);
 int rafting_step_wait_compact (rafting_engine_t* e, uint32_t slot);
 /* the dense outbox of the compact step last waited for in `slot` (every column that is non-NULL in out_host): the lossless
    fallback when the escape list overflowed */

@@ -5,6 +5,9 @@ with the engine — numpy only.
                  and, for steps with inbound requests, the request list (AppendEntries records + op escapes)
   decode_outbox  plan_c / rep_c / group columns / escape records  ->  the dense outbox columns
 
+A step over an active list (gids, rafting_step_begin_compact_active) has every column sized by len(gids), by position: the
+compact inbox and outbox carry the list, and the decoded outbox has the RAFTING_INBOX_COMPACT_GROUPS shape.
+
 The engine's own unpack / pack kernels (rafting_b200/csrc/compact.cuh) are the inverse of these two; tests/test_compact_gpu.py
 checks that a compact step, decoded, equals the dense step of the oracle bit for bit.
 """
@@ -18,8 +21,9 @@ U64 = np.uint64
 
 
 class CompactInbox:
-    def __init__(self, rows, n, F):
+    def __init__(self, rows, n, F, gids=None):
         self.rows, self.n, self.F = rows, n, F
+        self.gids = None if gids is None else np.ascontiguousarray(gids, dtype=np.uint32)   # active list: position i is gids[i]
         self.row_base = np.zeros(rows, dtype=np.int64)
         self.op_c = np.zeros((rows, n), dtype=np.uint32)
         self.op_unavail = None                                # [rows, n] uint16 when some follower is unavailable
@@ -63,8 +67,9 @@ class CompactRequests:
 
 
 class CompactOutbox:
-    def __init__(self, rows, n, F, esc_cap=4096):
+    def __init__(self, rows, n, F, esc_cap=4096, gids=None):
         self.rows, self.n, self.F, self.esc_cap = rows, n, F, esc_cap
+        self.gids = None if gids is None else np.ascontiguousarray(gids, dtype=np.uint32)   # active list: position i is gids[i]
         self.plan_c = np.zeros((rows, n, F), dtype=np.uint32)
         self.rep_c = np.zeros((rows, n), dtype=np.uint8)
         self.commit_index = np.zeros(n, dtype=np.int64)
@@ -108,11 +113,12 @@ class CompactOutbox:
         return t
 
 
-def outbox_in_block(block: np.ndarray, out_off, rows: int, n: int, F: int, esc_cap: int) -> CompactOutbox:
+def outbox_in_block(block: np.ndarray, out_off, rows: int, n: int, F: int, esc_cap: int, gids=None) -> CompactOutbox:
     """A CompactOutbox whose columns are views into ONE (pinned) uint8 block laid out by Engine.compact_layout: the engine then
-    brings a launch's whole outbox down with a single copy."""
+    brings a launch's whole outbox down with a single copy.  gids: the active list of the steps it will serve (n = len(gids))."""
     co = CompactOutbox.__new__(CompactOutbox)
     co.rows, co.n, co.F, co.esc_cap = rows, n, F, esc_cap
+    co.gids = None if gids is None else np.ascontiguousarray(gids, dtype=np.uint32)
     spec = (("plan_c", np.uint32, (rows, n, F)), ("rep_c", np.uint8, (rows, n)), ("commit_index", np.int64, (n,)),
             ("current_term", np.int64, (n,)), ("role_word", np.uint32, (n,)), ("incarnation", np.uint32, (n,)), ("err_word", np.uint32, (n,)),
             ("last_entry", abi.I64X2, (n,)), ("epoch", abi.I64X2, (n,)), ("counts", np.uint32, (4,)), ("esc", abi.CESC_OUT, (esc_cap,)))
@@ -128,6 +134,7 @@ def inbox_in_block(block: np.ndarray, in_off, ci: CompactInbox) -> CompactInbox:
     returns the CompactInbox whose columns are views into it: one copy up per launch."""
     out = CompactInbox.__new__(CompactInbox)
     out.rows, out.n, out.F = ci.rows, ci.n, ci.F
+    out.gids = getattr(ci, "gids", None)
     for k, name in enumerate(("row_base", "op_c", "op_unavail", "ev_c", "esc")):
         a = getattr(ci, name)
         if a is None or (name == "esc" and len(a) == 0):
@@ -193,7 +200,9 @@ def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray, elections:
 def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray | None, sent_inc: np.ndarray | None = None,
                  elections: bool = False, ballot_term: np.ndarray | None = None, ballot_inc: np.ndarray | None = None,
                  ballot_tags: np.ndarray | None = None) -> CompactInbox:
-    """ib: dense host inbox (any group ops, any lane events).
+    """ib: dense host inbox (any group ops, any lane events), over the whole shard or over an active list (ib.gids: the compact
+    inbox then carries the list, and every array below is per position of THIS step; a pump maps what it kept from the step
+    that planned by gid).
     tags[r, i, f]: the tag the RPC this event answers was sent under (plan_c of the step that emitted it); None = no acks yet.
     sent_term[i] / sent_inc[i]: the term those RPCs carried and the incarnation of the role object that sent them (the group's
     current_term / incarnation columns of the step that planned them).  The incarnation is not on the wire — the engine keeps
@@ -209,9 +218,7 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     vote replies in (r, i) answer (the decoded ballot columns of that step); a reply whose incarnation differs travels in
     full."""
     rows, n, F = ib.rows, ib.n, ib.F
-    if ib.gids is not None:
-        raise ValueError("the compact path is dense (no active list)")
-    c = CompactInbox(rows, n, F)
+    c = CompactInbox(rows, n, F, gids=ib.gids)
     ek = (ib.ev_meta & U64(0xF)).astype(np.int64) if ib.ev_meta is not None else np.zeros((rows, n, F), np.int64)
     has_op = ib.op_meta is not None
     ok = (ib.op_meta & U64(0xFF)) if has_op else None
@@ -289,11 +296,16 @@ def decode_outbox(co: CompactOutbox, G: int | None = None, elections: bool = Fal
     """The dense outbox a compact step stands for (rep_term / ballots / escaped plans come from the escape list).
     elections: the step was begun with abi.COMPACT_ELECTIONS, so plan_c lanes of kind CPLAN_PREVOTE / CPLAN_VOTE are ballots.
     prev_term: the step was begun with abi.COMPACT_PREV_TERM, so a lane of kind CPLAN_AE_PREV_TERM is an AE plan whose
-    prevLogTerm lies dterm below the group's term."""
+    prevLogTerm lies dterm below the group's term.
+    An active outbox (co.gids) decodes to the RAFTING_INBOX_COMPACT_GROUPS shape: group columns [n] by position, and o.gids."""
     rows, n, F = co.rows, co.n, co.F
     if int(co.counts[0]) > co.esc_cap:
         raise OverflowError("escape list overflow: fetch the dense outbox (rafting_step_fetch_dense)")
+    active = getattr(co, "gids", None)
+    if active is not None and G is not None and G != n:
+        raise ValueError("an active outbox has n group entries by position")
     o = abi.Outbox(rows, n, F, n if G is None else G)
+    o.gids = active
     pc = co.plan_c.astype(np.uint64)
     kind = (pc & U64(7)).astype(np.int64)
     older = (kind == abi.CPLAN_AE_PREV_TERM) if prev_term else np.zeros(kind.shape, bool)

@@ -42,25 +42,33 @@ struct COutD {                                   // device view of rafting_coutb
     bool compact_replies;                        // rep_c bits 6 / 7 (steps begun with a request list)
 };
 
+// the active list of a step begun with rafting_step_begin_compact_active (device copy): position i stands for gids[i]
+struct ActiveD { const uint32_t* gids; uint32_t n; };
+
 // EL: steps begun with RAFTING_COMPACT_ELECTIONS (vote replies as words, escaped words that free their tag)
-template <bool EL>
-__global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW out, const i64x2* __restrict__ table, const uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits) {
+// AL: steps over an active list.  One thread per (position, follower); the wire and the dense staging are positional, the
+//     in-flight table, its tag bitmap and the group tables stay indexed by gid (table stride G * F)
+template <bool EL, bool AL>
+__global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW out, const i64x2* __restrict__ table, const uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits, ActiveD act) {
     const uint32_t GF = T.G * T.F;
+    const uint32_t NF = AL ? act.n * T.F : GF;                       // lane slots of one row of the step
     const uint32_t t = blockIdx.x * 256u + threadIdx.x;
-    if (t >= GF) return;
-    const uint32_t g = t / T.F, f = t - g * T.F;
+    if (t >= NF) return;
+    const uint32_t i = t / T.F, f = t - i * T.F;                    // position in the step (the gid of a whole-shard step)
+    const uint32_t g = AL ? act.gids[i] : i;
+    const uint32_t s = AL ? g * T.F + f : t;                        // the lane's in-flight state
     if (in.ev_c) {
         const int64_t term_now = T.g_term[g];
-        uint32_t b = bits[t];
+        uint32_t b = bits[s];
         for (uint32_t r = 0; r < in.rows; r++) {
-            const size_t idx = (size_t)r * GF + t;
+            const size_t idx = (size_t)r * NF + t;
             const uint32_t w = in.ev_c[idx];
             const uint32_t kind = w & 0xfu;
             uint64_t em = 0;
             if (kind == RAFTING_EV_AE_ACK || kind == RAFTING_EV_IS_ACK) {
                 const uint32_t tag = (w >> 8) & 0xffu;
                 i64x2 el = {0, 0}; uint32_t inc = 0;
-                if (tag < (uint32_t)CTAGS) { el = table[(size_t)tag * GF + t]; inc = tinc[(size_t)tag * GF + t]; b &= ~(1u << tag); }
+                if (tag < (uint32_t)CTAGS) { el = table[(size_t)tag * GF + s]; inc = tinc[(size_t)tag * GF + s]; b &= ~(1u << tag); }
                 i64x2 tn; tn.x = ((w >> 7) & 1u) ? term_now : 0; tn.y = in.row_base[r] + (int64_t)(w >> 16);
                 em = (uint64_t)(w & 0x7fu) | ((uint64_t)inc << 32);         // kind | outcome | success | incarnation (from the table)
                 out.ev_tn[idx] = tn; out.ev_el[idx] = el;
@@ -68,7 +76,7 @@ __global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW o
                 if (kind == RAFTING_EV_PV_REPLY || kind == RAFTING_EV_RV_REPLY) {
                     // (ballot term, 0) and the asking role's incarnation wait under the tag; the reply's term is c below it
                     const uint32_t tag = RAFTING_CEV_VOTE_TAG(w);
-                    const int64_t bt = table[(size_t)tag * GF + t].x; const uint32_t inc = tinc[(size_t)tag * GF + t];
+                    const int64_t bt = table[(size_t)tag * GF + s].x; const uint32_t inc = tinc[(size_t)tag * GF + s];
                     b &= ~(1u << tag);
                     i64x2 tn; tn.x = ((w >> 4) & 3u) == RAFTING_OUT_OK ? (int64_t)((uint64_t)bt - RAFTING_CEV_VOTE_C(w)) : 0;
                     tn.y = in.row_base[r] + (int64_t)(w >> 16);
@@ -82,11 +90,11 @@ __global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW o
             }
             out.ev_meta[idx] = em;                                          // escaped / empty slots read as "no event" until patched
         }
-        bits[t] = b;
+        bits[s] = b;
     }
     if (f == 0 && (in.op_c || out.op_cd)) {
         for (uint32_t r = 0; r < in.rows; r++) {
-            const size_t gi = (size_t)r * T.G + g;
+            const size_t gi = (size_t)r * (AL ? act.n : T.G) + i;
             const uint32_t c = in.op_c ? in.op_c[gi] : 0u;
             out.op_meta[gi] = (uint64_t)RAFTING_OP_MAKE(c & 0xfu, 0u, (c >> 4) & 0xfffu);
             i64x2 nr; nr.x = in.row_base[r] + (int64_t)(c >> 16); nr.y = 0;
@@ -99,7 +107,7 @@ __global__ void __launch_bounds__(256) unpack_kernel(Tables T, CInD in, InboxW o
 
 // ---- the request list (rafting_creqs_t): records and op escapes, after unpack_kernel has written the op_c words ----
 struct CReqD {                                   // device view of rafting_creqs_t
-    uint32_t n_req, n_esc, slots;                // slots = rows * G
+    uint32_t n_req, n_esc, slots;                // slots = rows * n (n: the step's groups, max_groups or n_active)
     const rafting_creq_t* req; const rafting_cesc_op_t* esc;
     const int64_t* row_base; const uint32_t* op_c;
     uint32_t ent_count, pool_end;                // records' terms start at ent_count; the step's pool ends at pool_end
@@ -141,14 +149,14 @@ __device__ __forceinline__ void put_op(const InboxW& o, size_t gi, uint64_t meta
 // the order of the writes.
 // EL (RAFTING_COMPACT_ELECTIONS): a record with meta bits 11..12 set is a PreVote / RequestVote
 template <bool EL>
-__global__ void unpack_requests_kernel(CReqD q, InboxW o, uint32_t G) {
+__global__ void unpack_requests_kernel(CReqD q, InboxW o, uint32_t n) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if ((uint64_t)k >= (uint64_t)q.n_req + q.n_esc) return;
     const bool is_req = k < q.n_req;
     const uint32_t j = is_req ? k : k - q.n_req;
     const uint32_t slot = is_req ? q.req[j].slot : q.esc[j].slot;
     if (slot >= q.slots) return;
-    const uint32_t r = slot / G;
+    const uint32_t r = slot / n;
     bool bad = q.order[0] != 0 || (q.op_c && (q.op_c[slot] & 0xfu) != RAFTING_OP_NONE);
     if (is_req) {
         if constexpr (EL) {
@@ -236,24 +244,28 @@ __device__ __forceinline__ uint32_t ballot_lane_word(const OutboxD& in, size_t g
 }
 
 // PT: steps begun with RAFTING_COMPACT_PREV_TERM (an AE plan that breaks only the prevLogTerm rule becomes a kind-7 word)
-template <bool EL, bool PT>
-__global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, OutboxD in, COutD out, i64x2* __restrict__ table, uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits) {
+// AL: steps over an active list, as for unpack_kernel; the dense outbox's group columns are positional (COMPACT_GROUPS)
+template <bool EL, bool PT, bool AL>
+__global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, OutboxD in, COutD out, i64x2* __restrict__ table, uint32_t* __restrict__ tinc, uint32_t* __restrict__ bits, ActiveD act) {
     const uint32_t GF = T.G * T.F;
+    const uint32_t N = AL ? act.n : T.G, NF = AL ? act.n * T.F : GF;
     const uint32_t t = blockIdx.x * 256u + threadIdx.x;
-    if (t >= GF) return;
-    const uint32_t g = t / T.F, f = t - g * T.F;
+    if (t >= NF) return;
+    const uint32_t i = t / T.F, f = t - i * T.F;
+    const uint32_t g = AL ? act.gids[i] : i;
+    const uint32_t s = AL ? g * T.F + f : t;
     // the group's end-of-step snapshot: what the compact plan fields are relative to
-    const int64_t commit_end = in.commit_index[g], term_end = in.current_term[g];
-    const uint32_t inc_end = in.incarnation[g];
-    const i64x2 last_end = in.last_entry[g], epoch_end = T.g_epoch[g];
-    uint32_t b = bits[t];
+    const int64_t commit_end = in.commit_index[i], term_end = in.current_term[i];
+    const uint32_t inc_end = in.incarnation[i];
+    const i64x2 last_end = in.last_entry[i], epoch_end = T.g_epoch[g];
+    uint32_t b = bits[s];
     if (in.plan_meta) {
         for (uint32_t r = 0; r < rows; r++) {
-            const size_t idx = (size_t)r * GF + t;
+            const size_t idx = (size_t)r * NF + t;
             const uint64_t pm = in.plan_meta[idx];
             uint32_t pc = 0;
             if constexpr (EL) {
-                if (pm == 0) pc = ballot_lane_word(in, (size_t)r * T.G + g, T.F, term_end, inc_end, last_end, table + t, tinc + t, GF, b);
+                if (pm == 0) pc = ballot_lane_word(in, (size_t)r * N + i, T.F, term_end, inc_end, last_end, table + s, tinc + s, GF, b);
             }
             if (pm != 0) {
                 const uint32_t kind = RAFTING_PLM_KIND(pm), count = RAFTING_PLM_COUNT(pm);
@@ -264,7 +276,7 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
                     const uint32_t fr = ~b;
                     if (fr) {
                         tag = (uint32_t)__ffs((int)fr) - 1u; b |= 1u << tag;
-                        i64x2 v; v.x = pe; v.y = lc.x; table[(size_t)tag * GF + t] = v; tinc[(size_t)tag * GF + t] = RAFTING_PLM_INC(pm);
+                        i64x2 v; v.x = pe; v.y = lc.x; table[(size_t)tag * GF + s] = v; tinc[(size_t)tag * GF + s] = RAFTING_PLM_INC(pm);
                     }
                 }
                 const uint64_t dcommit = (uint64_t)commit_end - (uint64_t)lc.y;
@@ -292,14 +304,14 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
         }
     } else if constexpr (EL) {
         for (uint32_t r = 0; r < rows; r++)
-            out.plan_c[(size_t)r * GF + t] = ballot_lane_word(in, (size_t)r * T.G + g, T.F, term_end, inc_end, last_end, table + t, tinc + t, GF, b);
+            out.plan_c[(size_t)r * NF + t] = ballot_lane_word(in, (size_t)r * N + i, T.F, term_end, inc_end, last_end, table + s, tinc + s, GF, b);
     } else {
-        for (uint32_t r = 0; r < rows; r++) out.plan_c[(size_t)r * GF + t] = 0;
+        for (uint32_t r = 0; r < rows; r++) out.plan_c[(size_t)r * NF + t] = 0;
     }
-    bits[t] = b;
+    bits[s] = b;
     if (f == 0) {
         for (uint32_t r = 0; r < rows; r++) {
-            const size_t gi = (size_t)r * T.G + g;
+            const size_t gi = (size_t)r * N + i;
             const uint32_t rm = in.rep_meta ? in.rep_meta[gi] : 0u;
             uint32_t rc = RAFTING_REP_ERR(rm);
             if (RAFTING_REP_VALID(rm)) {
@@ -321,8 +333,8 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
                 if (bm != 0) { atomicAdd(out.counts + 1, 1u); const i64x2 bl = in.ballot_last[gi]; put_escape(out, RAFTING_CESC_BALLOT, (uint32_t)gi, bm, in.ballot_term[gi], bl.x, bl.y, 0, 0); }
             }
         }
-        out.commit_index[g] = commit_end; out.current_term[g] = term_end; out.role_word[g] = in.role_word[g];
-        out.incarnation[g] = inc_end; out.err_word[g] = in.err_word[g]; out.last_entry[g] = last_end; out.epoch[g] = epoch_end;
+        out.commit_index[i] = commit_end; out.current_term[i] = term_end; out.role_word[i] = in.role_word[i];
+        out.incarnation[i] = inc_end; out.err_word[i] = in.err_word[i]; out.last_entry[i] = last_end; out.epoch[i] = epoch_end;
     }
 }
 
@@ -406,8 +418,10 @@ extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot
     return rafting_step_begin_compact_ex(e, slot, in, reqs, out, 0u);
 }
 
-extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
-                                             const rafting_coutbox_t* out, uint32_t flags) {
+// One compact step in `slot`: over the whole shard (gids == nullptr, n = G), or over the n groups gids[0 .. n) that the caller
+// has checked (strictly increasing, each < G).  Every wire column and every dense staging column holds n groups per row.
+static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
+                         const rafting_coutbox_t* out, uint32_t flags, uint32_t n_active, const uint32_t* gids) {
     using namespace rafting;
     if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
     if (flags & ~(RAFTING_COMPACT_ELECTIONS | RAFTING_COMPACT_PREV_TERM)) return fail(RAFTING_E_INVAL, "unknown compact step flags 0x%x", flags);
@@ -431,16 +445,18 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
     HostPath* H = hp(e); Slot& S = H->slot[slot];
     if (S.leased) return fail(RAFTING_E_BUSY, "slot %u is held by an outstanding lease", slot);
     if (S.inflight) return fail(RAFTING_E_BUSY, "slot %u has a step in flight", slot);
-    const size_t rows = in->rows, G = e->G, F = e->F;
+    const bool list = gids != nullptr;
+    const size_t rows = in->rows, n = list ? n_active : e->G, F = e->F;       // n: groups per row of the step
     if (rows == 0 || rows > e->cfg.max_rows) return fail(RAFTING_E_CAPACITY, "rows %zu beyond max_rows %u", rows, e->cfg.max_rows);
     const size_t n_req = has_reqs ? reqs->n_req : 0, n_oesc = has_reqs ? reqs->n_op_esc : 0;
-    if (has_reqs && (uint64_t)rows * G * F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
-    if (n_req > rows * G || n_oesc > rows * G || n_req > 0x7fffffffu)
-        return fail(RAFTING_E_INVAL, "a request list longer than rows * G cannot be strictly increasing");
+    if (has_reqs && (uint64_t)rows * n * F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
+    if (n_req > rows * n || n_oesc > rows * n || n_req > 0x7fffffffu)
+        return fail(RAFTING_E_INVAL, "a request list longer than rows * n cannot be strictly increasing");
     const size_t ent_esc = has_reqs ? reqs->ent_count : 0, pool = has_reqs ? ent_esc + reqs->req_entries : 0;
-    const Layout LD = make_layout(rows, G, F, G, 0, 0);                        // dense staging the step kernel works on (the
-                                                                               // entry pool lives in the request block)
-    const CLayout LC = compact_layout(rows, G, F, in->n_esc, out->esc_cap);
+    // dense staging the step kernel works on (the entry pool lives in the request block); with an active list its group
+    // columns are positional (RAFTING_INBOX_COMPACT_GROUPS) and the list itself travels in its gids column
+    const Layout LD = make_layout(rows, n, F, n, list ? n : 0, 0);
+    const CLayout LC = compact_layout(rows, n, F, in->n_esc, out->esc_cap);
     const CRLayout LR = compact_req_layout(n_req, n_oesc, ent_esc);
     size_t scan_tmp = 0;
     if (n_req) CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n_req));
@@ -460,15 +476,15 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
                                in->op_c && in->ev_c;
         if (one_block) {
             const size_t span = in->n_esc ? LC.esc + (size_t)in->n_esc * sizeof(rafting_cesc_in_t)
-                                : (in->op_unavail ? LC.op_un + rows * G * 2 : LC.ev_c + rows * G * F * 4);
+                                : (in->op_unavail ? LC.op_un + rows * n * 2 : LC.ev_c + rows * n * F * 4);
             CU(cudaMemcpyAsync(S.cin.p, hb, span, cudaMemcpyHostToDevice, H->s_h2d));
             ci.op_c = (const uint32_t*)(S.cin.p + LC.op_c); ci.ev_c = (const uint32_t*)(S.cin.p + LC.ev_c);
             if (in->op_unavail) ci.op_unavail = (const uint16_t*)(S.cin.p + LC.op_un);
         } else {
             CU(cudaMemcpyAsync(S.cin.p + LC.row_base, in->row_base, rows * 8, cudaMemcpyHostToDevice, H->s_h2d));
-            if (in->op_c) { CU(cudaMemcpyAsync(S.cin.p + LC.op_c, in->op_c, rows * G * 4, cudaMemcpyHostToDevice, H->s_h2d)); ci.op_c = (const uint32_t*)(S.cin.p + LC.op_c); }
-            if (in->op_c && in->op_unavail) { CU(cudaMemcpyAsync(S.cin.p + LC.op_un, in->op_unavail, rows * G * 2, cudaMemcpyHostToDevice, H->s_h2d)); ci.op_unavail = (const uint16_t*)(S.cin.p + LC.op_un); }
-            if (in->ev_c) { CU(cudaMemcpyAsync(S.cin.p + LC.ev_c, in->ev_c, rows * G * F * 4, cudaMemcpyHostToDevice, H->s_h2d)); ci.ev_c = (const uint32_t*)(S.cin.p + LC.ev_c); }
+            if (in->op_c) { CU(cudaMemcpyAsync(S.cin.p + LC.op_c, in->op_c, rows * n * 4, cudaMemcpyHostToDevice, H->s_h2d)); ci.op_c = (const uint32_t*)(S.cin.p + LC.op_c); }
+            if (in->op_c && in->op_unavail) { CU(cudaMemcpyAsync(S.cin.p + LC.op_un, in->op_unavail, rows * n * 2, cudaMemcpyHostToDevice, H->s_h2d)); ci.op_unavail = (const uint16_t*)(S.cin.p + LC.op_un); }
+            if (in->ev_c) { CU(cudaMemcpyAsync(S.cin.p + LC.ev_c, in->ev_c, rows * n * F * 4, cudaMemcpyHostToDevice, H->s_h2d)); ci.ev_c = (const uint32_t*)(S.cin.p + LC.ev_c); }
             if (in->n_esc) CU(cudaMemcpyAsync(S.cin.p + LC.esc, in->esc, (size_t)in->n_esc * sizeof(rafting_cesc_in_t), cudaMemcpyHostToDevice, H->s_h2d));
         }
     }
@@ -483,10 +499,16 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
             if (ent_esc) CU(cudaMemcpyAsync(S.creq.p + LR.ent, reqs->ent_terms, ent_esc * 8, cudaMemcpyHostToDevice, H->s_h2d));
         }
     }
+    ActiveD act; act.gids = nullptr; act.n = (uint32_t)n;
+    if (list) {
+        act.gids = (const uint32_t*)(S.din.p + LD.in_off[0]);
+        CU(cudaMemcpyAsync((void*)act.gids, gids, n * 4, cudaMemcpyHostToDevice, H->s_h2d));
+    }
     CU(cudaEventRecord(S.ev_h2d, H->s_h2d));
     // ---- unpack -> step -> pack on the engine's stream ----
     InboxD di; memset(&di, 0, sizeof(di));
-    di.rows = (uint32_t)rows; di.n = (uint32_t)G; di.flags = has_reqs ? 0u : RAFTING_INBOX_NO_REQUESTS;
+    di.rows = (uint32_t)rows; di.n = (uint32_t)n; di.flags = has_reqs ? 0u : RAFTING_INBOX_NO_REQUESTS;
+    if (list) { di.gids = act.gids; di.flags |= RAFTING_INBOX_COMPACT_GROUPS; }
     if (in->op_c || has_reqs) {
         di.op_meta = (const uint64_t*)(S.din.p + LD.in_off[2]); di.op_nr = (const i64x2*)(S.din.p + LD.in_off[3]);
         if (in->op_unavail || has_reqs) di.op_ab = (const i64x2*)(S.din.p + LD.in_off[4]);   // else nobody is unavailable
@@ -515,7 +537,7 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
     co.incarnation = (uint32_t*)(S.cout.p + LC.inc); co.err_word = (uint32_t*)(S.cout.p + LC.err); co.last_entry = (i64x2*)(S.cout.p + LC.last);
     co.epoch = (i64x2*)(S.cout.p + LC.epoch); co.counts = (uint32_t*)(S.cout.p + LC.counts);
     co.esc = (rafting_cesc_out_t*)(S.cout.p + LC.esc_out); co.esc_cap = out->esc_cap; co.compact_replies = reqs != nullptr;
-    const uint32_t GF = (uint32_t)(G * F), blocks = (GF + 255u) / 256u;
+    const uint32_t NF = (uint32_t)(n * F), blocks = (NF + 255u) / 256u;
     CU(cudaStreamWaitEvent(e->stream, S.ev_h2d, 0));
     CU(cudaMemsetAsync(dov.flags, 0, 16, e->stream));
     CU(cudaMemsetAsync(co.counts, 0, 16, e->stream));
@@ -523,13 +545,13 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
     dw.op_meta = (uint64_t*)di.op_meta; dw.op_nr = (i64x2*)di.op_nr; dw.op_ab = (i64x2*)di.op_ab;
     dw.ev_meta = (uint64_t*)di.ev_meta; dw.ev_tn = (i64x2*)di.ev_tn; dw.ev_el = (i64x2*)di.ev_el;
     dw.op_cd = (i64x2*)di.op_cd; dw.op_e = (int64_t*)di.op_e; dw.ent_terms = (int64_t*)di.ent_terms;
-    if (el) unpack_kernel<true><<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits);
-    else unpack_kernel<false><<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits);
-    if (in->ev_c == nullptr && in->n_esc) CU(cudaMemsetAsync((void*)di.ev_meta, 0, rows * G * F * 8, e->stream));
-    if (in->n_esc) unpack_escapes_kernel<<<(in->n_esc + 255u) / 256u, 256, 0, e->stream>>>(ci, dw, (uint32_t)(rows * G * F));
+    auto* unpack = list ? (el ? unpack_kernel<true, true> : unpack_kernel<false, true>) : (el ? unpack_kernel<true, false> : unpack_kernel<false, false>);
+    unpack<<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits, act);
+    if (in->ev_c == nullptr && in->n_esc) CU(cudaMemsetAsync((void*)di.ev_meta, 0, rows * n * F * 8, e->stream));
+    if (in->n_esc) unpack_escapes_kernel<<<(in->n_esc + 255u) / 256u, 256, 0, e->stream>>>(ci, dw, (uint32_t)(rows * n * F));
     if (has_reqs) {
         CReqD q;
-        q.n_req = (uint32_t)n_req; q.n_esc = (uint32_t)n_oesc; q.slots = (uint32_t)(rows * G);
+        q.n_req = (uint32_t)n_req; q.n_esc = (uint32_t)n_oesc; q.slots = (uint32_t)(rows * n);
         q.req = (const rafting_creq_t*)(S.creq.p + LR.req); q.esc = (const rafting_cesc_op_t*)(S.creq.p + LR.esc);
         q.row_base = ci.row_base; q.op_c = ci.op_c;
         q.ent_count = (uint32_t)ent_esc; q.pool_end = (uint32_t)pool;
@@ -539,14 +561,15 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
         creq_prepare_kernel<<<(most + 255u) / 256u, 256, 0, e->stream>>>(q);
         if (n_req) { size_t tb = scan_tmp; CU(cub::DeviceScan::ExclusiveSum(S.creqw.p + w_tmp, tb, q.counts, q.offs, (int)n_req, e->stream)); }
         const uint32_t rq_blocks = (uint32_t)((n_req + n_oesc + 255u) / 256u);
-        if (el) unpack_requests_kernel<true><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)G);
-        else unpack_requests_kernel<false><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)G);
+        if (el) unpack_requests_kernel<true><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)n);
+        else unpack_requests_kernel<false><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)n);
     }
     CU(cudaGetLastError());
     rc = launch_step(e, di, dov, e->stream);
     if (rc) { cudaStreamSynchronize(H->s_h2d); return rc; }
-    auto* pack = el ? (pt ? pack_kernel<true, true> : pack_kernel<true, false>) : (pt ? pack_kernel<false, true> : pack_kernel<false, false>);
-    pack<<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits);
+    auto* pack = list ? (el ? (pt ? pack_kernel<true, true, true> : pack_kernel<true, false, true>) : (pt ? pack_kernel<false, true, true> : pack_kernel<false, false, true>))
+                      : (el ? (pt ? pack_kernel<true, true, false> : pack_kernel<true, false, false>) : (pt ? pack_kernel<false, true, false> : pack_kernel<false, false, false>));
+    pack<<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits, act);
     CU(cudaGetLastError());
     CU(cudaEventRecord(S.ev_kernel, e->stream));
     // ---- D2H: every wire column + the counters; the escape list only when the counters say it holds something ----
@@ -564,15 +587,15 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
             CU(cudaMemcpyAsync(hb, S.cout.p, LC.esc_out + (size_t)esc_inline * sizeof(rafting_cesc_out_t), cudaMemcpyDeviceToHost, H->s_d2h));
             counts_land = out->counts;
         } else {
-            CU(cudaMemcpyAsync(out->plan_c, co.plan_c, rows * G * F * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->rep_c, co.rep_c, rows * G, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->commit_index, co.commit_index, G * 8, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->current_term, co.current_term, G * 8, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->role_word, co.role_word, G * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->incarnation, co.incarnation, G * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->err_word, co.err_word, G * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->last_entry, co.last_entry, G * 16, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->epoch, co.epoch, G * 16, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->plan_c, co.plan_c, rows * n * F * 4, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->rep_c, co.rep_c, rows * n, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->commit_index, co.commit_index, n * 8, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->current_term, co.current_term, n * 8, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->role_word, co.role_word, n * 4, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->incarnation, co.incarnation, n * 4, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->err_word, co.err_word, n * 4, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->last_entry, co.last_entry, n * 16, cudaMemcpyDeviceToHost, H->s_d2h));
+            CU(cudaMemcpyAsync(out->epoch, co.epoch, n * 16, cudaMemcpyDeviceToHost, H->s_d2h));
             CU(cudaMemcpyAsync(S.chout.p, co.counts, 16, cudaMemcpyDeviceToHost, H->s_d2h));
             // the first escape records always travel with the columns (a steady-state launch produces a handful): fetching them
             // on demand at wait time would have to drain the D2H stream, i.e. wait for the copies of every LATER launch as well
@@ -587,9 +610,29 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
     S.dev_out.ballot_meta = dov.ballot_meta; S.dev_out.ballot_term = dov.ballot_term; S.dev_out.ballot_last = (rafting_i64x2_t*)dov.ballot_last;
     S.dev_out.commit_index = dov.commit_index; S.dev_out.current_term = dov.current_term; S.dev_out.role_word = dov.role_word;
     S.dev_out.incarnation = dov.incarnation; S.dev_out.err_word = dov.err_word; S.dev_out.last_entry = (rafting_i64x2_t*)dov.last_entry;
-    S.rows_ = rows; S.n_ = G;
+    S.rows_ = rows; S.n_ = n; S.gcols_ = n;
     S.inflight = true;
     return RAFTING_OK;
+}
+
+extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
+                                             const rafting_coutbox_t* out, uint32_t flags) {
+    return compact_begin(e, slot, in, reqs, out, flags, 0, nullptr);
+}
+
+// The list is checked in full before anything is enqueued: a lane's tag bitmap must have exactly one owning thread, and the
+// in-flight table is indexed by gid, so a duplicate or an id past max_groups would race on it or index past it.
+extern "C" int rafting_step_begin_compact_active(rafting_engine_t* e, uint32_t slot, uint32_t n_active, const uint32_t* gids,
+                                                 const rafting_cinbox_t* in, const rafting_creqs_t* reqs, const rafting_coutbox_t* out,
+                                                 uint32_t flags) {
+    if (!e || !gids) return fail(RAFTING_E_INVAL, "bad argument");
+    if (n_active == 0) return fail(RAFTING_E_INVAL, "an active list holds at least one group");
+    if (n_active > e->G) return fail(RAFTING_E_CAPACITY, "n_active %u > max_groups %u", n_active, e->G);
+    for (uint32_t k = 0; k < n_active; k++) {
+        if (gids[k] >= e->G) return fail(RAFTING_E_INVAL, "gids[%u] = %u is not below max_groups", k, gids[k]);
+        if (k > 0 && gids[k] <= gids[k - 1]) return fail(RAFTING_E_INVAL, "gids must be strictly increasing (gids[%u] = %u)", k, gids[k]);
+    }
+    return compact_begin(e, slot, in, reqs, out, flags, n_active, gids);
 }
 
 extern "C" int rafting_step_wait_compact(rafting_engine_t* e, uint32_t slot) {
@@ -619,7 +662,7 @@ extern "C" int rafting_step_fetch_dense(rafting_engine_t* e, uint32_t slot, cons
         const ColDesc& c = OUT_COLS[k];
         void* h = out_ptr(out, c); void* d = out_ptr(&S.dev_out, c);
         if (!h || !d) continue;
-        CU(cudaMemcpyAsync(h, d, col_bytes(c, S.rows_, S.n_, e->F, e->G, 0, 0), cudaMemcpyDeviceToHost, H->s_d2h));
+        CU(cudaMemcpyAsync(h, d, col_bytes(c, S.rows_, S.n_, e->F, S.gcols_, 0, 0), cudaMemcpyDeviceToHost, H->s_d2h));
     }
     CU(cudaStreamSynchronize(H->s_d2h));
     return RAFTING_OK;

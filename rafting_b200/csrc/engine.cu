@@ -476,6 +476,7 @@ struct Slot {
     uint32_t lease_gen = 0;
     // of the step in flight (for the sparse columns fetched at wait time)
     rafting_outbox_t host_out; rafting_outbox_t dev_out; size_t rows_ = 0, n_ = 0; const uint32_t* flags_host = nullptr;
+    size_t gcols_ = 0;                        // compact steps: entries of a per-group column (max_groups, or n_active)
 };
 struct HostPath {
     Slot slot[RAFTING_HOST_SLOTS];

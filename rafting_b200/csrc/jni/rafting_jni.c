@@ -121,6 +121,12 @@ JNIEXPORT void JNICALL FN(stepBeginCompactEx)(JNIEnv* env, jclass k, jlong h, ji
     CHECK(rafting_step_begin_compact_ex(ENG(h), (uint32_t)slot, (const rafting_cinbox_t*)BUF(cin), (const rafting_creqs_t*)BUF(creqs),
                                         (const rafting_coutbox_t*)BUF(cout), (uint32_t)flags));
 }
+/* ... over an active list: nActive uint32 gids in a direct buffer, every column of cinbox / coutbox sized by nActive */
+JNIEXPORT void JNICALL FN(stepBeginCompactActive)(JNIEnv* env, jclass k, jlong h, jint slot, jint nActive, jobject gids, jobject cin, jobject creqs,
+                                                  jobject cout, jint flags) {
+    CHECK(rafting_step_begin_compact_active(ENG(h), (uint32_t)slot, (uint32_t)nActive, (const uint32_t*)BUF(gids), (const rafting_cinbox_t*)BUF(cin),
+                                            (const rafting_creqs_t*)BUF(creqs), (const rafting_coutbox_t*)BUF(cout), (uint32_t)flags));
+}
 JNIEXPORT void JNICALL FN(stepWaitCompact)(JNIEnv* env, jclass k, jlong h, jint slot) { CHECK(rafting_step_wait_compact(ENG(h), (uint32_t)slot)); }
 JNIEXPORT void JNICALL FN(stepFetchDense)(JNIEnv* env, jclass k, jlong h, jint slot, jobject outStruct) {
     CHECK(rafting_step_fetch_dense(ENG(h), (uint32_t)slot, (const rafting_outbox_t*)BUF(outStruct)));

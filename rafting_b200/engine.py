@@ -38,7 +38,7 @@ EXPORTS = [
     "rafting_comm_init", "rafting_comm_init_all", "rafting_comm_unique_id", "rafting_allgather_commit", "rafting_allgather_commit_from",
     "rafting_allgather_commit_all", "rafting_allgather_last", "rafting_restore_async", "rafting_state_save", "rafting_state_load", "rafting_step_device_seq", "rafting_engine_stream",
     "rafting_engine_counters", "rafting_abi_sizes", "rafting_checkpoint", "rafting_restore",
-    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
+    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_step_begin_compact_active", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
     "rafting_log_config", "rafting_log_append", "rafting_log_read", "rafting_log_gather", "rafting_log_trim", "rafting_log_stats",
     "rafting_log_store_open", "rafting_log_sync", "rafting_log_mark", "rafting_log_recovered", "rafting_log_export_kv", "rafting_log_store_stats",
 ]
@@ -117,6 +117,8 @@ def lib():
                                                      C.POINTER(abi.COutboxC)]
         L.rafting_step_begin_compact_ex.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(abi.CInboxC), C.POINTER(abi.CReqsC),
                                                     C.POINTER(abi.COutboxC), C.c_uint32]
+        L.rafting_step_begin_compact_active.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(abi.CInboxC),
+                                                        C.POINTER(abi.CReqsC), C.POINTER(abi.COutboxC), C.c_uint32]
         L.rafting_compact_req_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 4)]
         L.rafting_step_wait_compact.argtypes = [C.c_void_p, C.c_uint32]
         L.rafting_compact_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 6),
@@ -246,12 +248,26 @@ class Engine:
         _check(lib().rafting_step_begin_compact_ex(self._h, slot, C.byref(cin_c), None if reqs_c is None else C.byref(reqs_c),
                                                    C.byref(cout_c), flags), "rafting_step_begin_compact_ex")
 
+    def step_begin_compact_active(self, slot: int, gids: np.ndarray, cin_c: abi.CInboxC, reqs_c: abi.CReqsC | None,
+                                  cout_c: abi.COutboxC, flags: int = 0):
+        """rafting_step_begin_compact_active: a compact step over the groups gids (uint32, strictly increasing, each below
+        max_groups); every column of cin_c / cout_c holds len(gids) groups per row, by position.  gids must stay alive until
+        the wait."""
+        if gids.dtype != np.uint32 or not gids.flags.c_contiguous:
+            raise TypeError("gids must be a contiguous uint32 array")
+        _check(lib().rafting_step_begin_compact_active(self._h, slot, len(gids), gids.ctypes.data if len(gids) else None,
+                                                       C.byref(cin_c), None if reqs_c is None else C.byref(reqs_c),
+                                                       C.byref(cout_c), flags), "rafting_step_begin_compact_active")
+
     def step_compact(self, cin, cout, slot: int = 0, reqs=None, flags: int = 0):
         """Synchronous compact step: cin / cout are rafting_b200.compact.CompactInbox / CompactOutbox, reqs a
         rafting_b200.compact.CompactRequests (None: rafting_step_begin_compact).  flags (rafting_step_begin_compact_ex):
         abi.COMPACT_ELECTIONS carries ballots, vote replies and vote requests compact, abi.COMPACT_PREV_TERM AE plans whose
-        prevLogTerm lies 1..8 below the group's term; the two combine."""
-        if flags:
+        prevLogTerm lies 1..8 below the group's term; the two combine.  An inbox with an active list (cin.gids) runs through
+        rafting_step_begin_compact_active."""
+        if getattr(cin, "gids", None) is not None:
+            self.step_begin_compact_active(slot, cin.gids, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags)
+        elif flags:
             self.step_begin_compact_ex(slot, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags)
         elif reqs is None:
             self.step_begin_compact(slot, cin.as_c(), cout.as_c())

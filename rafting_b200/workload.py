@@ -65,10 +65,30 @@ def election_step(w: WlCfg, phase: int, prev_out_c, inbox_c, on_device=False, st
         raise RuntimeError(f"rafting_wl_election_step rc={rc}")
 
 
-def leader_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None) -> abi.Inbox:
-    """Host (numpy) inbox of one leader-steady-state step."""
-    ib = abi.Inbox(w.rows, w.n, w.F)
+def _over(w: WlCfg, gids) -> tuple[WlCfg, dict]:
+    """w over the active list gids (None: w itself): a copy with n = len(gids), and the Inbox arguments of such a step.  The
+    inbox carries RAFTING_INBOX_COMPACT_GROUPS, so the previous outbox's group columns are read by position, as a compact
+    active step returns them; every draw stays keyed by the gid, so a group sees the same stream with or without a list."""
+    if gids is None:
+        return w, {}
+    v = WlCfg()
+    C.pointer(v)[0] = w
+    v.n = len(gids)
+    return v, dict(gids=gids)
+
+
+def _listed(ib: abi.Inbox) -> abi.Inbox:
+    if ib.gids is not None:
+        ib.flags |= abi.INBOX_COMPACT_GROUPS
+    return ib
+
+
+def leader_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None, gids=None) -> abi.Inbox:
+    """Host (numpy) inbox of one leader-steady-state step (over the active list gids when given, see _over)."""
+    w, kw = _over(w, gids)
+    ib = abi.Inbox(w.rows, w.n, w.F, **kw)
     ib.flags = abi.INBOX_NO_REQUESTS
+    _listed(ib)
     ic = ib.as_c()
     ic.op_cd = None
     ic.op_e = None
@@ -91,9 +111,10 @@ def election_inbox_host(w: WlCfg, phase: int, prev_out: abi.Outbox | None) -> ab
 POOL_TERMS = 256 * 50
 
 
-def vote_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None) -> abi.Inbox:
-    """config #3 (RequestVote storm, PreVote on): one host inbox."""
-    ib = abi.Inbox(w.rows, w.n, w.F)
+def vote_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None, gids=None) -> abi.Inbox:
+    """config #3 (RequestVote storm, PreVote on): one host inbox (over the active list gids when given, see _over)."""
+    w, kw = _over(w, gids)
+    ib = _listed(abi.Inbox(w.rows, w.n, w.F, **kw))
     rc = _bind().rafting_wl_vote_step(C.byref(w), step, None if prev_out is None else C.byref(prev_out.as_c()),
                                       C.byref(ib.as_c()), 0, None)
     if rc:
@@ -101,9 +122,11 @@ def vote_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None) -> abi.Inb
     return ib
 
 
-def mixed_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None) -> abi.Inbox:
-    """config #5 (mixed leader churn + InstallSnapshot catch-up): one host inbox."""
-    ib = abi.Inbox(w.rows, w.n, w.F, ent_cap=POOL_TERMS)
+def mixed_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None, gids=None) -> abi.Inbox:
+    """config #5 (mixed leader churn + InstallSnapshot catch-up): one host inbox (over the active list gids when given, see
+    _over)."""
+    w, kw = _over(w, gids)
+    ib = _listed(abi.Inbox(w.rows, w.n, w.F, ent_cap=POOL_TERMS, **kw))
     _bind().rafting_wl_fill_term_pool(ib.ent_terms.ctypes.data, POOL_TERMS, 0, None)
     ib.ent_count = POOL_TERMS
     rc = _bind().rafting_wl_mixed_step(C.byref(w), step, None if prev_out is None else C.byref(prev_out.as_c()),
