@@ -626,6 +626,54 @@ int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot /* 0..3 */,
 int rafting_step_begin_compact_active(rafting_engine_t* e, uint32_t slot /* 0..3 */, uint32_t n_active, const uint32_t* gids /* host */,
                                       const rafting_cinbox_t* in_host, const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host,
                                       uint32_t flags);
+/* TIMERS on the compact path.  Raft's timers (RaftRoutine's TimerTicket: a follower's / candidate's election timeout, a leader's
+ * keepAlive, RaftRoutine.java:53-130) fire on a SWEEP ROW: row r of a step with row_now[r] = t != 0 gives every group of the
+ * step whose timer is due at t the implied RAFTING_OP_TIMEOUT in that row's op slot, where due means
+ *        alive && (leader ? timer <= t : timer > 0 && timer != INT64_MAX && timer <= t)
+ * The deadlines live in HBM and move inside steps (resetTimer on AppendEntries, votes and role changes, counter-based draws,
+ * muted timers), so a pump does not track them; it asks the engine which groups are due and lists those.
+ *
+ * rafting_step_begin_compact_sweep: the compact step (whole shard when gids == NULL, else over the active list gids[0 .. n_active),
+ *   checked as rafting_step_begin_compact_active checks it) that stands for the dense step with row_now = sweep (host, [rows];
+ *   0 = not a sweep row; NULL = no sweep row).  Its wire columns, flags (0, 1, 4 or 5), request list and outbox mean what they mean
+ *   for rafting_step_begin_compact_ex / _active; rafting_step_wait_compact and rafting_step_fetch_dense serve it.
+ *   * a sweep row's op slot belongs to the sweep: its op_c words are ignored, as the dense step ignores op_meta there, and a
+ *     request record or op escape whose slot lies on a sweep row is refused (RAFTING_E_INVAL, nothing enqueued, slot free).
+ *   * a step that holds only a sweep (no op_c, no ev_c, no request) is legal: its heartbeats, ballots and replies come back in
+ *     plan_c / rep_c and the escape list like those of any op.
+ *   * the sweep column travels up in the same copy as the active list (alone for a whole-shard step).
+ *
+ * rafting_timers_due_begin / _wait: the gids a sweep row at t = until_ms would fire, over the whole shard, as of every step begun
+ *   before the query (it is enqueued on the engine's step stream, behind them; begin does not synchronise).
+ *   * gids_out receives the due gids in strictly increasing order.  n_due is the full count: when n_due > cap only the first cap
+ *     gids are written (the lowest ones) — never silently, the count says so; query again with a larger buffer, or list the
+ *     first cap now and the rest after the next query.  cap == 0 asks for the count and the next deadline only.
+ *   * gids_out should be pinned (cudaHostAlloc / registered): the device then writes it directly.  Any other host memory works
+ *     through a pinned staging block of the query slot, copied into gids_out at the wait.  It must stay valid until the wait.
+ *   * next_deadline_ms: the earliest deadline after until_ms that a later sweep would fire (the least timer > until_ms of an
+ *     alive leader, or of an alive follower / candidate whose timer is armed: > 0 and != INT64_MAX); INT64_MAX if there is none.
+ *     An idle pump sleeps until then.
+ *   * query slots 0..RAFTING_HOST_SLOTS-1 are independent of the step slots; each holds one query until its wait
+ *     (RAFTING_E_BUSY otherwise).  The table is the engine's, so the query serves whole-shard and active, dense and compact steps.
+ *
+ * PIPELINING RULE.  A pump encodes step k+1 while steps k-d+1 .. k (d >= 0) are in flight, its sweep times never decrease.  With
+ * Q = the due list of a query begun after step k-d, at until = the last sweep time of step k+1, the list
+ *        Q  u  event gids of steps k-d+1 .. k+1        (event gid: a group op outside the sweep rows, or a lane event)
+ * holds every group that a whole-shard sweep would fire in step k+1, and listing exactly those groups leaves the shard as the
+ * whole-shard step would.  For a group g outside it:
+ *   * g has no event in steps k-d+1 .. k+1, and Q says it is not due at until; the predicate is monotone in t, so it was not due
+ *     at any earlier sweep time of those steps either;
+ *   * a group without events whose timer is not due is left untouched by a step (listed or not, a sweep row passes it by), so
+ *     step by step g keeps the state Q was computed from, and is not due at step k+1.
+ * Listing more is always safe: a listed group that is not due is left untouched by a sweep row.  So the lists of the steps in
+ * flight may be added as well, but they need not be, and should not: each list would then contain the one before it.
+ * (A whole-shard in-flight step counts as an event of every group.) */
+int rafting_step_begin_compact_sweep(rafting_engine_t* e, uint32_t slot /* 0..3 */, uint32_t n_active, const uint32_t* gids /* NULL = whole shard */,
+                                     const int64_t* sweep /* [rows], host; 0 = not a sweep row */,
+                                     const rafting_cinbox_t* in_host, const rafting_creqs_t* reqs, const rafting_coutbox_t* out_host,
+                                     uint32_t flags);
+int rafting_timers_due_begin(rafting_engine_t* e, uint32_t slot /* 0..3 */, int64_t until_ms, uint32_t* gids_out /* host [cap] */, uint32_t cap);
+int rafting_timers_due_wait (rafting_engine_t* e, uint32_t slot, uint32_t* n_due, int64_t* next_deadline_ms);
 int rafting_step_wait_compact (rafting_engine_t* e, uint32_t slot);
 /* the dense outbox of the compact step last waited for in `slot` (every column that is non-NULL in out_host): the lossless
    fallback when the escape list overflowed */

@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librafting_b200.so")
 SOURCES = ["engine.cu"]
-HEADERS = ["step_kernel.cuh", "step_body.inc", "seglog.cuh", "compact.cuh", "pair_kernel.cuh", "handlers.cuh", "tables.cuh",
+HEADERS = ["step_kernel.cuh", "step_body.inc", "seglog.cuh", "compact.cuh", "timers.cuh", "pair_kernel.cuh", "handlers.cuh", "tables.cuh",
            os.path.join("..", "..", "include", "rafting_b200.h")]
 # the synthetic-stream generator (the simulated peers) is NOT part of the product library: tests, bench and the CPU
 # reference arm load it on its own, so a process that times the CPU port never maps librafting_b200.so

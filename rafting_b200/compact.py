@@ -4,6 +4,7 @@ with the engine — numpy only.
   encode_inbox   dense lane events / group ops  ->  ev_c / op_c / row_base (+ escape records for whatever breaks a compact rule)
                  and, for steps with inbound requests, the request list (AppendEntries records + op escapes)
   decode_outbox  plan_c / rep_c / group columns / escape records  ->  the dense outbox columns
+  encode_inbox(sweep=True) also carries the dense inbox's row_now as the sweep column of rafting_step_begin_compact_sweep
 
 A step over an active list (gids, rafting_step_begin_compact_active) has every column sized by len(gids), by position: the
 compact inbox and outbox carry the list, and the decoded outbox has the RAFTING_INBOX_COMPACT_GROUPS shape.
@@ -197,9 +198,25 @@ def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray, elections:
     return CompactRequests(req, op_esc, np.concatenate(terms).astype(np.int64) if terms else None), listed
 
 
+def sweep_column(ib: abi.Inbox) -> np.ndarray:
+    """The sweep column of a compact step that stands for the dense inbox ib: its row_now (int64 [rows]; zeros without one)."""
+    if ib.row_now is None:
+        return np.zeros(ib.rows, dtype=np.int64)
+    return np.ascontiguousarray(ib.row_now[:ib.rows], dtype=np.int64)
+
+
+def _without_sweep_row_ops(ib: abi.Inbox, on: np.ndarray) -> abi.Inbox:
+    """ib with every group op of the sweep rows `on` removed: the step ignores them, and a request record there is refused."""
+    out = abi.Inbox.__new__(abi.Inbox)
+    out.__dict__.update(ib.__dict__)
+    out.op_meta = ib.op_meta.copy()
+    out.op_meta[on] = 0
+    return out
+
+
 def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray | None, sent_inc: np.ndarray | None = None,
                  elections: bool = False, ballot_term: np.ndarray | None = None, ballot_inc: np.ndarray | None = None,
-                 ballot_tags: np.ndarray | None = None) -> CompactInbox:
+                 ballot_tags: np.ndarray | None = None, sweep: bool = False) -> CompactInbox:
     """ib: dense host inbox (any group ops, any lane events), over the whole shard or over an active list (ib.gids: the compact
     inbox then carries the list, and every array below is per position of THIS step; a pump maps what it kept from the step
     that planned by gid).
@@ -216,7 +233,17 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     ballot_tags[r, i, f] (CompactOutbox.ballot_tags() of the step that emitted the ballot; None = no compact ballot, every
     vote reply travels in full).  ballot_term[r, i] / ballot_inc[r, i]: the term and the asking incarnation of the ballot the
     vote replies in (r, i) answer (the decoded ballot columns of that step); a reply whose incarnation differs travels in
-    full."""
+    full.
+    sweep: the inbox of a step begun with rafting_step_begin_compact_sweep.  `.sweep` holds ib.row_now (sweep_column), and the
+    group ops of the sweep rows are dropped: the step ignores them there, and a request record on a sweep row is refused.
+    Off (the default), row_now is not encoded: the compact step has no sweep rows."""
+    if sweep:
+        col = sweep_column(ib)
+        if ib.op_meta is not None and (col != 0).any():
+            ib = _without_sweep_row_ops(ib, col != 0)
+        c = encode_inbox(ib, tags, sent_term, sent_inc, elections, ballot_term, ballot_inc, ballot_tags)
+        c.sweep = col
+        return c
     rows, n, F = ib.rows, ib.n, ib.F
     c = CompactInbox(rows, n, F, gids=ib.gids)
     ek = (ib.ev_meta & U64(0xF)).astype(np.int64) if ib.ev_meta is not None else np.zeros((rows, n, F), np.int64)

@@ -420,15 +420,19 @@ extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot
 
 // One compact step in `slot`: over the whole shard (gids == nullptr, n = G), or over the n groups gids[0 .. n) that the caller
 // has checked (strictly increasing, each < G).  Every wire column and every dense staging column holds n groups per row.
+// sweep (host, [rows], may be null): the step's row_now column (rafting_step_begin_compact_sweep).
 static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
-                         const rafting_coutbox_t* out, uint32_t flags, uint32_t n_active, const uint32_t* gids) {
+                         const rafting_coutbox_t* out, uint32_t flags, uint32_t n_active, const uint32_t* gids,
+                         const int64_t* sweep = nullptr) {
     using namespace rafting;
     if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
     if (flags & ~(RAFTING_COMPACT_ELECTIONS | RAFTING_COMPACT_PREV_TERM)) return fail(RAFTING_E_INVAL, "unknown compact step flags 0x%x", flags);
     const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0, pt = (flags & RAFTING_COMPACT_PREV_TERM) != 0;
     const bool has_reqs = reqs && (reqs->n_req || reqs->n_op_esc);
-    if (!in->row_base || (!in->op_c && !in->ev_c && !has_reqs))
-        return fail(RAFTING_E_INVAL, "compact inbox needs row_base and at least one of op_c / ev_c / a request");
+    bool has_sweep = false;
+    if (sweep) for (uint32_t r = 0; r < in->rows && r < e->cfg.max_rows; r++) has_sweep |= sweep[r] != 0;
+    if (!in->row_base || (!in->op_c && !in->ev_c && !has_reqs && !has_sweep))
+        return fail(RAFTING_E_INVAL, "compact inbox needs row_base and at least one of op_c / ev_c / a request / a sweep row");
     if (reqs && ((reqs->n_req && !reqs->req) || (reqs->n_op_esc && !reqs->op_esc) || (reqs->ent_count && !reqs->ent_terms)))
         return fail(RAFTING_E_INVAL, "request list: a count without its array");
     if (reqs && (uint64_t)reqs->ent_count + reqs->req_entries > e->cfg.entry_pool_cap)
@@ -452,6 +456,15 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     if (has_reqs && (uint64_t)rows * n * F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
     if (n_req > rows * n || n_oesc > rows * n || n_req > 0x7fffffffu)
         return fail(RAFTING_E_INVAL, "a request list longer than rows * n cannot be strictly increasing");
+    if (has_sweep) {
+        // a sweep row's op slot belongs to the sweep: the step would drop a request placed there without a trace
+        for (size_t k = 0; k < n_req + n_oesc; k++) {
+            const uint32_t at = k < n_req ? reqs->req[k].slot : reqs->op_esc[k - n_req].slot;
+            if (at < rows * n && sweep[at / n] != 0)
+                return fail(RAFTING_E_INVAL, "%s %zu (slot %u) lies on sweep row %zu", k < n_req ? "request record" : "op escape",
+                            k < n_req ? k : k - n_req, at, (size_t)(at / n));
+        }
+    }
     const size_t ent_esc = has_reqs ? reqs->ent_count : 0, pool = has_reqs ? ent_esc + reqs->req_entries : 0;
     // dense staging the step kernel works on (the entry pool lives in the request block); with an active list its group
     // columns are positional (RAFTING_INBOX_COMPACT_GROUPS) and the list itself travels in its gids column
@@ -464,6 +477,10 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     if ((rc = blk_reserve(S.din, LD.in_total, false)) || (rc = blk_reserve(S.dout, LD.out_total, false)) ||
         (rc = blk_reserve(S.cin, LC.in_total, false)) || (rc = blk_reserve(S.cout, LC.out_total, false)) ||
         (rc = blk_reserve(S.chout, 256, true))) return rc;
+    // the sweep column travels in the copy of the list (whole shard: alone), staged in the slot's pinned block so that the copy
+    // is asynchronous whatever memory the caller's column lives in
+    const size_t sweep_at = list ? LD.in_off[1] - LD.in_off[0] : 0;
+    if (has_sweep && (rc = blk_reserve(S.chin, sweep_at + rows * 8, true))) return rc;
     if (has_reqs && ((rc = blk_reserve(S.creq, LR.ent + pool * 8, false)) || (rc = blk_reserve(S.creqw, w_tmp + scan_tmp, false)))) return rc;
     // ---- H2D: the wire columns as they are ----
     CInD ci; ci.rows = (uint32_t)rows; ci.n_esc = in->n_esc;
@@ -500,8 +517,12 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
         }
     }
     ActiveD act; act.gids = nullptr; act.n = (uint32_t)n;
-    if (list) {
-        act.gids = (const uint32_t*)(S.din.p + LD.in_off[0]);
+    if (list) act.gids = (const uint32_t*)(S.din.p + LD.in_off[0]);
+    if (has_sweep) {                                                           // [gids | pad] sweep: one copy
+        if (list) memcpy(S.chin.p, gids, n * 4);
+        memcpy(S.chin.p + sweep_at, sweep, rows * 8);
+        CU(cudaMemcpyAsync(S.din.p + LD.in_off[1] - sweep_at, S.chin.p, sweep_at + rows * 8, cudaMemcpyHostToDevice, H->s_h2d));
+    } else if (list) {
         CU(cudaMemcpyAsync((void*)act.gids, gids, n * 4, cudaMemcpyHostToDevice, H->s_h2d));
     }
     CU(cudaEventRecord(S.ev_h2d, H->s_h2d));
@@ -509,6 +530,7 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     InboxD di; memset(&di, 0, sizeof(di));
     di.rows = (uint32_t)rows; di.n = (uint32_t)n; di.flags = has_reqs ? 0u : RAFTING_INBOX_NO_REQUESTS;
     if (list) { di.gids = act.gids; di.flags |= RAFTING_INBOX_COMPACT_GROUPS; }
+    if (has_sweep) di.row_now = (const int64_t*)(S.din.p + LD.in_off[1]);
     if (in->op_c || has_reqs) {
         di.op_meta = (const uint64_t*)(S.din.p + LD.in_off[2]); di.op_nr = (const i64x2*)(S.din.p + LD.in_off[3]);
         if (in->op_unavail || has_reqs) di.op_ab = (const i64x2*)(S.din.p + LD.in_off[4]);   // else nobody is unavailable
@@ -530,7 +552,7 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     dov.incarnation = (uint32_t*)(S.dout.p + LD.out_off[12]); dov.err_word = (uint32_t*)(S.dout.p + LD.out_off[13]);
     dov.last_entry = (i64x2*)(S.dout.p + LD.out_off[14]);
     dov.flags = (uint32_t*)(S.dout.p + LD.flags_off);
-    if (!in->op_c && !has_reqs) { dov.rep_meta = nullptr; dov.rep_term = nullptr; dov.plan_meta = nullptr; dov.plan_pp = nullptr; dov.plan_lc = nullptr; dov.plan_epoch = nullptr; }
+    if (!in->op_c && !has_reqs && !has_sweep) { dov.rep_meta = nullptr; dov.rep_term = nullptr; dov.plan_meta = nullptr; dov.plan_pp = nullptr; dov.plan_lc = nullptr; dov.plan_epoch = nullptr; }
     COutD co;
     co.plan_c = (uint32_t*)(S.cout.p + LC.plan_c); co.rep_c = (uint8_t*)(S.cout.p + LC.rep_c);
     co.commit_index = (int64_t*)(S.cout.p + LC.commit); co.current_term = (int64_t*)(S.cout.p + LC.term); co.role_word = (uint32_t*)(S.cout.p + LC.role);
@@ -622,9 +644,7 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
 
 // The list is checked in full before anything is enqueued: a lane's tag bitmap must have exactly one owning thread, and the
 // in-flight table is indexed by gid, so a duplicate or an id past max_groups would race on it or index past it.
-extern "C" int rafting_step_begin_compact_active(rafting_engine_t* e, uint32_t slot, uint32_t n_active, const uint32_t* gids,
-                                                 const rafting_cinbox_t* in, const rafting_creqs_t* reqs, const rafting_coutbox_t* out,
-                                                 uint32_t flags) {
+static int check_active_list(rafting_engine_t* e, uint32_t n_active, const uint32_t* gids) {
     if (!e || !gids) return fail(RAFTING_E_INVAL, "bad argument");
     if (n_active == 0) return fail(RAFTING_E_INVAL, "an active list holds at least one group");
     if (n_active > e->G) return fail(RAFTING_E_CAPACITY, "n_active %u > max_groups %u", n_active, e->G);
@@ -632,7 +652,22 @@ extern "C" int rafting_step_begin_compact_active(rafting_engine_t* e, uint32_t s
         if (gids[k] >= e->G) return fail(RAFTING_E_INVAL, "gids[%u] = %u is not below max_groups", k, gids[k]);
         if (k > 0 && gids[k] <= gids[k - 1]) return fail(RAFTING_E_INVAL, "gids must be strictly increasing (gids[%u] = %u)", k, gids[k]);
     }
+    return RAFTING_OK;
+}
+extern "C" int rafting_step_begin_compact_active(rafting_engine_t* e, uint32_t slot, uint32_t n_active, const uint32_t* gids,
+                                                 const rafting_cinbox_t* in, const rafting_creqs_t* reqs, const rafting_coutbox_t* out,
+                                                 uint32_t flags) {
+    if (int rc = check_active_list(e, n_active, gids)) return rc;
     return compact_begin(e, slot, in, reqs, out, flags, n_active, gids);
+}
+
+// The dense step with row_now = sweep, over the whole shard (gids == NULL) or an active list
+extern "C" int rafting_step_begin_compact_sweep(rafting_engine_t* e, uint32_t slot, uint32_t n_active, const uint32_t* gids, const int64_t* sweep,
+                                                const rafting_cinbox_t* in, const rafting_creqs_t* reqs, const rafting_coutbox_t* out,
+                                                uint32_t flags) {
+    if (gids) { if (int rc = check_active_list(e, n_active, gids)) return rc; }
+    else n_active = 0;
+    return compact_begin(e, slot, in, reqs, out, flags, n_active, gids, sweep);
 }
 
 extern "C" int rafting_step_wait_compact(rafting_engine_t* e, uint32_t slot) {

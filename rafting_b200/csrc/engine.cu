@@ -94,6 +94,7 @@ struct rafting_engine {
     std::vector<void*> shadow;         // rafting_checkpoint copies, parallel to dev_allocs (null for scratch)
     bool alloc_state = true;           // what dalloc marks new allocations as
     struct CompactState* compact = nullptr;   // in-flight table of the compact host path (compact.cuh), created on first use
+    struct DuePath* due = nullptr;             // query slots of rafting_timers_due_begin (timers.cuh), created on first use
 };
 
 template <typename T>
@@ -112,6 +113,7 @@ static int dalloc(rafting_engine* e, T** p, size_t count) {
 static void rafting_hostpath_release(rafting_engine* e);
 static void seglog_release(rafting_engine* e);
 static void compact_release(rafting_engine* e);
+static void due_release(rafting_engine* e);
 static int compact_state(rafting_engine* e);
 static int quiesce_for_table_edit(rafting_engine* e, const char* who);
 extern "C" uint32_t rafting_abi_version(void) { return RAFTING_ABI_VERSION; }
@@ -175,6 +177,7 @@ extern "C" int rafting_engine_destroy(rafting_engine_t* e) {
     for (void* p : e->dev_allocs) cudaFree(p);
     for (void* p : e->shadow) if (p) cudaFree(p);
     compact_release(e);
+    due_release(e);
     rafting_hostpath_release(e);
     seglog_release(e);
     if (e->ev_seg) cudaEventDestroy(e->ev_seg);
@@ -1152,4 +1155,5 @@ extern "C" int rafting_abi_sizes(uint32_t* out, uint32_t n) {
 }
 
 #include "compact.cuh"
+#include "timers.cuh"
 #include "seglog.cuh"

@@ -127,7 +127,31 @@ JNIEXPORT void JNICALL FN(stepBeginCompactActive)(JNIEnv* env, jclass k, jlong h
     CHECK(rafting_step_begin_compact_active(ENG(h), (uint32_t)slot, (uint32_t)nActive, (const uint32_t*)BUF(gids), (const rafting_cinbox_t*)BUF(cin),
                                             (const rafting_creqs_t*)BUF(creqs), (const rafting_coutbox_t*)BUF(cout), (uint32_t)flags));
 }
+/* ... with sweep rows: `sweep` holds rows int64 sweep times (0 = not a sweep row); gids null = the whole shard */
+JNIEXPORT void JNICALL FN(stepBeginCompactSweep)(JNIEnv* env, jclass k, jlong h, jint slot, jint nActive, jobject gids, jobject sweep, jobject cin,
+                                                 jobject creqs, jobject cout, jint flags) {
+    CHECK(rafting_step_begin_compact_sweep(ENG(h), (uint32_t)slot, (uint32_t)nActive, (const uint32_t*)BUF(gids), (const int64_t*)BUF(sweep),
+                                           (const rafting_cinbox_t*)BUF(cin), (const rafting_creqs_t*)BUF(creqs), (const rafting_coutbox_t*)BUF(cout),
+                                           (uint32_t)flags));
+}
 JNIEXPORT void JNICALL FN(stepWaitCompact)(JNIEnv* env, jclass k, jlong h, jint slot) { CHECK(rafting_step_wait_compact(ENG(h), (uint32_t)slot)); }
+/* the groups a sweep at untilMs would fire: gidsOut (cap uint32) is filled at the wait; result = {nDue, nextDeadlineMs} */
+JNIEXPORT void JNICALL FN(timersDueBegin)(JNIEnv* env, jclass k, jlong h, jint slot, jlong untilMs, jobject gidsOut, jint cap) {
+    CHECK(rafting_timers_due_begin(ENG(h), (uint32_t)slot, (int64_t)untilMs, (uint32_t*)BUF(gidsOut), (uint32_t)cap));
+}
+JNIEXPORT void JNICALL FN(timersDueWait)(JNIEnv* env, jclass k, jlong h, jint slot, jlongArray result) {
+    uint32_t n = 0; int64_t next = 0;
+    int rc = rafting_timers_due_wait(ENG(h), (uint32_t)slot, &n, &next);
+    if (rc) { throw_status(env, rc); return; }
+    if (!result || (*env)->GetArrayLength(env, result) < 2) {
+        jclass c = (*env)->FindClass(env, "java/lang/IllegalArgumentException");
+        if (c) (*env)->ThrowNew(env, c, "timersDueWait: the result array needs 2 elements {nDue, nextDeadlineMs}");
+        return;
+    }
+    jlong* r = (*env)->GetLongArrayElements(env, result, NULL);
+    r[0] = (jlong)n; r[1] = (jlong)next;
+    (*env)->ReleaseLongArrayElements(env, result, r, 0);
+}
 JNIEXPORT void JNICALL FN(stepFetchDense)(JNIEnv* env, jclass k, jlong h, jint slot, jobject outStruct) {
     CHECK(rafting_step_fetch_dense(ENG(h), (uint32_t)slot, (const rafting_outbox_t*)BUF(outStruct)));
 }

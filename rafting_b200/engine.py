@@ -38,7 +38,7 @@ EXPORTS = [
     "rafting_comm_init", "rafting_comm_init_all", "rafting_comm_unique_id", "rafting_allgather_commit", "rafting_allgather_commit_from",
     "rafting_allgather_commit_all", "rafting_allgather_last", "rafting_restore_async", "rafting_state_save", "rafting_state_load", "rafting_step_device_seq", "rafting_engine_stream",
     "rafting_engine_counters", "rafting_abi_sizes", "rafting_checkpoint", "rafting_restore",
-    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_step_begin_compact_active", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
+    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_step_begin_compact_active", "rafting_step_begin_compact_sweep", "rafting_timers_due_begin", "rafting_timers_due_wait", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
     "rafting_log_config", "rafting_log_append", "rafting_log_read", "rafting_log_gather", "rafting_log_trim", "rafting_log_stats",
     "rafting_log_store_open", "rafting_log_sync", "rafting_log_mark", "rafting_log_recovered", "rafting_log_export_kv", "rafting_log_store_stats",
 ]
@@ -119,6 +119,10 @@ def lib():
                                                     C.POINTER(abi.COutboxC), C.c_uint32]
         L.rafting_step_begin_compact_active.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(abi.CInboxC),
                                                         C.POINTER(abi.CReqsC), C.POINTER(abi.COutboxC), C.c_uint32]
+        L.rafting_step_begin_compact_sweep.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(abi.CInboxC),
+                                                       C.POINTER(abi.CReqsC), C.POINTER(abi.COutboxC), C.c_uint32]
+        L.rafting_timers_due_begin.argtypes = [C.c_void_p, C.c_uint32, C.c_int64, C.c_void_p, C.c_uint32]
+        L.rafting_timers_due_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_int64)]
         L.rafting_compact_req_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 4)]
         L.rafting_step_wait_compact.argtypes = [C.c_void_p, C.c_uint32]
         L.rafting_compact_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 6),
@@ -259,13 +263,66 @@ class Engine:
                                                        C.byref(cin_c), None if reqs_c is None else C.byref(reqs_c),
                                                        C.byref(cout_c), flags), "rafting_step_begin_compact_active")
 
+    def step_begin_compact_sweep(self, slot: int, sweep: np.ndarray, cin_c: abi.CInboxC, reqs_c: abi.CReqsC | None,
+                                 cout_c: abi.COutboxC, flags: int = 0, gids: np.ndarray | None = None):
+        """rafting_step_begin_compact_sweep: the compact step that stands for the dense step with row_now = sweep (int64 [rows],
+        0 = not a sweep row), over the whole shard (gids None) or the active list gids.  sweep and gids must stay alive until
+        the wait."""
+        if sweep.dtype != np.int64 or not sweep.flags.c_contiguous:
+            raise TypeError("sweep must be a contiguous int64 array")
+        if len(sweep) < cin_c.rows:
+            raise ValueError(f"sweep holds {len(sweep)} rows, the inbox {cin_c.rows}")
+        if gids is not None and (gids.dtype != np.uint32 or not gids.flags.c_contiguous):
+            raise TypeError("gids must be a contiguous uint32 array")
+        n, g = (0, None) if gids is None else (len(gids), gids.ctypes.data if len(gids) else None)
+        _check(lib().rafting_step_begin_compact_sweep(self._h, slot, n, g, sweep.ctypes.data, C.byref(cin_c),
+                                                      None if reqs_c is None else C.byref(reqs_c), C.byref(cout_c), flags),
+               "rafting_step_begin_compact_sweep")
+
+    def timers_due_begin(self, slot: int, until_ms: int, out: np.ndarray | int | None, cap: int | None = None):
+        """rafting_timers_due_begin: enqueue the query "which groups would a sweep at until_ms fire" behind every step begun
+        so far.  out: a uint32 array (or the address of pinned host memory, with cap) that receives the due gids; it must stay
+        alive until timers_due_wait."""
+        if out is None:
+            if cap:
+                raise ValueError("a cap without a buffer")
+            ptr, cap = None, 0
+        elif isinstance(out, int):
+            if cap is None:
+                raise ValueError("an address needs its cap (the number of uint32 it holds)")
+            ptr = out
+        else:
+            if out.dtype != np.uint32 or not out.flags.c_contiguous:
+                raise TypeError("out must be a contiguous uint32 array")
+            if cap is not None and cap > len(out):
+                raise ValueError(f"cap {cap} exceeds the buffer's {len(out)} entries")
+            ptr, cap = (out.ctypes.data if len(out) else None), len(out) if cap is None else cap
+        _check(lib().rafting_timers_due_begin(self._h, slot, until_ms, ptr, cap), "rafting_timers_due_begin")
+
+    def timers_due_wait(self, slot: int) -> tuple[int, int]:
+        """-> (n_due, next_deadline_ms).  n_due may exceed the buffer's cap: then only its first cap gids were written."""
+        n, nxt = C.c_uint32(), C.c_int64()
+        _check(lib().rafting_timers_due_wait(self._h, slot, C.byref(n), C.byref(nxt)), "rafting_timers_due_wait")
+        return n.value, nxt.value
+
+    def timers_due(self, until_ms: int, slot: int = 0) -> tuple[np.ndarray, int]:
+        """Synchronous: (the gids a sweep at until_ms would fire, the next deadline after it)."""
+        out = np.zeros(self.G, dtype=np.uint32)
+        self.timers_due_begin(slot, until_ms, out)
+        n, nxt = self.timers_due_wait(slot)
+        return out[:n].copy(), nxt
+
     def step_compact(self, cin, cout, slot: int = 0, reqs=None, flags: int = 0):
         """Synchronous compact step: cin / cout are rafting_b200.compact.CompactInbox / CompactOutbox, reqs a
         rafting_b200.compact.CompactRequests (None: rafting_step_begin_compact).  flags (rafting_step_begin_compact_ex):
         abi.COMPACT_ELECTIONS carries ballots, vote replies and vote requests compact, abi.COMPACT_PREV_TERM AE plans whose
         prevLogTerm lies 1..8 below the group's term; the two combine.  An inbox with an active list (cin.gids) runs through
-        rafting_step_begin_compact_active."""
-        if getattr(cin, "gids", None) is not None:
+        rafting_step_begin_compact_active, and one encoded with a sweep column (compact.encode_inbox(sweep=True)) through
+        rafting_step_begin_compact_sweep."""
+        if getattr(cin, "sweep", None) is not None:
+            self.step_begin_compact_sweep(slot, cin.sweep, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags,
+                                          gids=getattr(cin, "gids", None))
+        elif getattr(cin, "gids", None) is not None:
             self.step_begin_compact_active(slot, cin.gids, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags)
         elif flags:
             self.step_begin_compact_ex(slot, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags)
