@@ -487,7 +487,8 @@ typedef struct rafting_coutbox {
     rafting_cesc_out_t* esc;         /* [esc_cap] */
     uint32_t  esc_cap, _pad;
     uint32_t* counts;                /* [4] escape records produced (may exceed esc_cap: then use rafting_step_fetch_dense),
-                                        ballots, valid replies, reserved */
+                                        ballots, valid replies, and for rafting_step_begin_compact_due the number of due groups
+                                        outside the host's list (0 for every other step) */
 } rafting_coutbox_t;
 /* Byte offsets of the wire columns inside ONE block per direction, as the engine lays them out on the device.  A caller that
    carves its pinned inbox / outbox out of one block with these offsets gets ONE copy up and ONE copy down per launch instead
@@ -674,6 +675,34 @@ int rafting_step_begin_compact_sweep(rafting_engine_t* e, uint32_t slot /* 0..3 
                                      uint32_t flags);
 int rafting_timers_due_begin(rafting_engine_t* e, uint32_t slot /* 0..3 */, int64_t until_ms, uint32_t* gids_out /* host [cap] */, uint32_t cap);
 int rafting_timers_due_wait (rafting_engine_t* e, uint32_t slot, uint32_t* n_due, int64_t* next_deadline_ms);
+/* DUE STEPS: the step finds its own due groups, so a pump lists only the groups it has events for, at any depth of pipelining.
+ * rafting_step_begin_compact_due is a sweep step over a list of n = n_host + cap positions:
+ *   * positions 0 .. n_host-1 are gids, checked as an active list is (strictly increasing, each < max_groups), except that
+ *     n_host = 0 is allowed (a pure timer tick);
+ *   * positions n_host .. n-1, the TAIL, are chosen on the device on the step stream right before the step, from the state the
+ *     step itself sees (whatever is in flight): first the groups outside gids that a sweep at t = max(sweep[r]) would fire, lowest
+ *     gids first, up to cap of them; then FILLERS, groups outside gids that are not due at t, lowest first, until the tail holds
+ *     cap entries.  Each of the two parts is strictly increasing; the tail and the whole list are not, and need not be: no
+ *     kernel of a step depends on the order of its list, only on its uniqueness (one owner per lane's tag bitmap).
+ *     Fillers keep n a host-known number, and they are exact: a listed group with no event whose timer is not due is left
+ *     untouched by a sweep row.
+ *   * counts[3] of the outbox is the full number of due groups outside gids.  If counts[3] <= cap, tail positions n_host ..
+ *     n_host + counts[3] - 1 hold due groups and the rest fillers, and the step leaves the shard exactly as the whole-shard
+ *     compact sweep step with the same events would.  If counts[3] > cap it is exactly the sweep step over gids u tail; the due
+ *     groups left over stay due, untouched, and the next step finds them (raise cap).
+ *   * tail_out (host [cap]) receives the tail; it is valid after rafting_step_wait_compact.
+ *   * every column and slot is positional with n = n_host + cap, both ways, as for rafting_step_begin_compact_active
+ *     (rafting_compact_layout(rows, n_host + cap, F, ...)); the host leaves the tail positions of op_c, op_unavail and ev_c empty.
+ *     flags is 0, 1, 4 or 5; rafting_step_fetch_dense returns the COMPACT_GROUPS-shaped dense outbox with n = n_host + cap.
+ *   * refused with nothing enqueued and the slot free: a request record or op escape at a position >= n_host or on a sweep row,
+ *     a lane escape record at a tail position, no sweep row, cap = 0, and n_host + cap > max_groups (RAFTING_E_CAPACITY: there
+ *     would not be enough fillers).
+ * Use it rather than rafting_step_begin_compact_sweep over the PIPELINING RULE's list when steps are in flight: the rule must
+ * list every event gid of the steps in flight as well, and at d = 3 that covers most of a heartbeat-driven shard. */
+int rafting_step_begin_compact_due(rafting_engine_t* e, uint32_t slot /* 0..3 */, uint32_t n_host, const uint32_t* gids /* host, [n_host] */,
+                                   uint32_t cap, const int64_t* sweep /* [rows], host */,
+                                   const rafting_cinbox_t* in_host, const rafting_creqs_t* reqs,
+                                   const rafting_coutbox_t* out_host, uint32_t* tail_out /* host [cap] */, uint32_t flags);
 int rafting_step_wait_compact (rafting_engine_t* e, uint32_t slot);
 /* the dense outbox of the compact step last waited for in `slot` (every column that is non-NULL in out_host): the lossless
    fallback when the escape list overflowed */

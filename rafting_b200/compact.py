@@ -205,6 +205,23 @@ def sweep_column(ib: abi.Inbox) -> np.ndarray:
     return np.ascontiguousarray(ib.row_now[:ib.rows], dtype=np.int64)
 
 
+def due_inbox(ib: abi.Inbox, cap: int) -> abi.Inbox:
+    """The dense inbox of a step begun with rafting_step_begin_compact_due: ib over the host's list ib.gids (positional, the
+    COMPACT_GROUPS shape; ib.n may be 0) followed by `cap` empty tail positions, whose groups the device chooses.  Encode it
+    with encode_inbox(..., sweep=True): every column and slot is then positional with n = len(ib.gids) + cap, and the compact
+    inbox's gids stay the host's list.  After the wait, CompactOutbox.gids = gids followed by the tail (Engine.step_compact_due)."""
+    out = abi.Inbox.__new__(abi.Inbox)
+    out.__dict__.update(ib.__dict__)
+    out.n = ib.n + cap
+    out.gids = np.ascontiguousarray(ib.gids if ib.gids is not None else np.zeros(0, np.uint32), dtype=np.uint32)
+    for name in ("op_meta", "op_nr", "op_ab", "op_cd", "op_e", "ev_meta", "ev_tn", "ev_el"):
+        col = getattr(ib, name)
+        if col is not None:
+            pad = np.zeros((col.shape[0], cap) + col.shape[2:], dtype=col.dtype)
+            setattr(out, name, np.ascontiguousarray(np.concatenate([col, pad], axis=1)))
+    return out
+
+
 def _without_sweep_row_ops(ib: abi.Inbox, on: np.ndarray) -> abi.Inbox:
     """ib with every group op of the sweep rows `on` removed: the step ignores them, and a request record there is refused."""
     out = abi.Inbox.__new__(abi.Inbox)

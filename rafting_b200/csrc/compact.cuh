@@ -418,12 +418,19 @@ extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot
     return rafting_step_begin_compact_ex(e, slot, in, reqs, out, 0u);
 }
 
+// the device-chosen tail of a step begun with rafting_step_begin_compact_due (timers.cuh)
+struct DueTail { uint32_t n_host, cap; uint32_t* tail_out; };
+static int tail_scratch_bytes(uint32_t G, size_t* bytes);
+static int tail_select(rafting_engine* e, uint8_t* scratch, int64_t until, uint32_t* list, uint32_t n_host, uint32_t cap, uint32_t* n_due);
+
 // One compact step in `slot`: over the whole shard (gids == nullptr, n = G), or over the n groups gids[0 .. n) that the caller
 // has checked (strictly increasing, each < G).  Every wire column and every dense staging column holds n groups per row.
 // sweep (host, [rows], may be null): the step's row_now column (rafting_step_begin_compact_sweep).
+// due (rafting_step_begin_compact_due): gids holds due->n_host entries and n_active = n_host + cap; the device writes the
+// rest of the list before unpack_kernel reads it.
 static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
                          const rafting_coutbox_t* out, uint32_t flags, uint32_t n_active, const uint32_t* gids,
-                         const int64_t* sweep = nullptr) {
+                         const int64_t* sweep = nullptr, const DueTail* due = nullptr) {
     using namespace rafting;
     if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
     if (flags & ~(RAFTING_COMPACT_ELECTIONS | RAFTING_COMPACT_PREV_TERM)) return fail(RAFTING_E_INVAL, "unknown compact step flags 0x%x", flags);
@@ -449,8 +456,9 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     HostPath* H = hp(e); Slot& S = H->slot[slot];
     if (S.leased) return fail(RAFTING_E_BUSY, "slot %u is held by an outstanding lease", slot);
     if (S.inflight) return fail(RAFTING_E_BUSY, "slot %u has a step in flight", slot);
-    const bool list = gids != nullptr;
+    const bool list = gids != nullptr || due != nullptr;
     const size_t rows = in->rows, n = list ? n_active : e->G, F = e->F;       // n: groups per row of the step
+    const size_t n_listed = due ? due->n_host : n;                            // entries of gids the host wrote
     if (rows == 0 || rows > e->cfg.max_rows) return fail(RAFTING_E_CAPACITY, "rows %zu beyond max_rows %u", rows, e->cfg.max_rows);
     const size_t n_req = has_reqs ? reqs->n_req : 0, n_oesc = has_reqs ? reqs->n_op_esc : 0;
     if (has_reqs && (uint64_t)rows * n * F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
@@ -465,6 +473,20 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
                             k < n_req ? k : k - n_req, at, (size_t)(at / n));
         }
     }
+    if (due) {
+        // the tail's groups are chosen on the device: nothing the host sends can name one of its positions
+        for (size_t k = 0; k < n_req + n_oesc; k++) {
+            const uint32_t at = k < n_req ? reqs->req[k].slot : reqs->op_esc[k - n_req].slot;
+            if (at < rows * n && at % n >= n_listed)
+                return fail(RAFTING_E_INVAL, "%s %zu (slot %u) lies at tail position %zu", k < n_req ? "request record" : "op escape",
+                            k < n_req ? k : k - n_req, at, (size_t)(at % n));
+        }
+        for (uint32_t k = 0; k < in->n_esc; k++) {
+            const uint32_t at = in->esc[k].slot;
+            if (at < rows * n * F && (at / F) % n >= n_listed)
+                return fail(RAFTING_E_INVAL, "escape record %u (slot %u) lies at tail position %zu", k, at, (size_t)((at / F) % n));
+        }
+    }
     const size_t ent_esc = has_reqs ? reqs->ent_count : 0, pool = has_reqs ? ent_esc + reqs->req_entries : 0;
     // dense staging the step kernel works on (the entry pool lives in the request block); with an active list its group
     // columns are positional (RAFTING_INBOX_COMPACT_GROUPS) and the list itself travels in its gids column
@@ -476,7 +498,9 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     const size_t w_counts = 256, w_offs = w_counts + ((n_req * 8 + 255) & ~(size_t)255), w_tmp = w_offs + ((n_req * 8 + 255) & ~(size_t)255);
     if ((rc = blk_reserve(S.din, LD.in_total, false)) || (rc = blk_reserve(S.dout, LD.out_total, false)) ||
         (rc = blk_reserve(S.cin, LC.in_total, false)) || (rc = blk_reserve(S.cout, LC.out_total, false)) ||
-        (rc = blk_reserve(S.chout, 256, true))) return rc;
+        (rc = blk_reserve(S.chout, 256 + (due ? (size_t)due->cap * 4 : 0), true))) return rc;
+    size_t tail_bytes = 0;
+    if (due && ((rc = tail_scratch_bytes(e->G, &tail_bytes)) || (rc = blk_reserve(S.ctail, tail_bytes, false)))) return rc;
     // the sweep column travels in the copy of the list (whole shard: alone), staged in the slot's pinned block so that the copy
     // is asynchronous whatever memory the caller's column lives in
     const size_t sweep_at = list ? LD.in_off[1] - LD.in_off[0] : 0;
@@ -519,7 +543,7 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     ActiveD act; act.gids = nullptr; act.n = (uint32_t)n;
     if (list) act.gids = (const uint32_t*)(S.din.p + LD.in_off[0]);
     if (has_sweep) {                                                           // [gids | pad] sweep: one copy
-        if (list) memcpy(S.chin.p, gids, n * 4);
+        if (list && n_listed) memcpy(S.chin.p, gids, n_listed * 4);
         memcpy(S.chin.p + sweep_at, sweep, rows * 8);
         CU(cudaMemcpyAsync(S.din.p + LD.in_off[1] - sweep_at, S.chin.p, sweep_at + rows * 8, cudaMemcpyHostToDevice, H->s_h2d));
     } else if (list) {
@@ -563,7 +587,14 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     CU(cudaStreamWaitEvent(e->stream, S.ev_h2d, 0));
     CU(cudaMemsetAsync(dov.flags, 0, 16, e->stream));
     CU(cudaMemsetAsync(co.counts, 0, 16, e->stream));
-    InboxW dw;                                                                 // unpack writes what the step kernel reads
+    if (due) {                                                                 // the tail of the list, and counts[3]
+        int64_t until = 0;
+        for (size_t r = 0; r < rows; r++) until = sweep[r] > until ? sweep[r] : until;
+        if ((rc = tail_select(e, S.ctail.p, until, (uint32_t*)act.gids, due->n_host, due->cap, co.counts + 3))) {
+            cudaStreamSynchronize(H->s_h2d); return rc;
+        }
+    }
+    InboxW dw;                                                                // unpack writes what the step kernel reads
     dw.op_meta = (uint64_t*)di.op_meta; dw.op_nr = (i64x2*)di.op_nr; dw.op_ab = (i64x2*)di.op_ab;
     dw.ev_meta = (uint64_t*)di.ev_meta; dw.ev_tn = (i64x2*)di.ev_tn; dw.ev_el = (i64x2*)di.ev_el;
     dw.op_cd = (i64x2*)di.op_cd; dw.op_e = (int64_t*)di.op_e; dw.ent_terms = (int64_t*)di.ent_terms;
@@ -624,8 +655,10 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
             if (esc_inline) CU(cudaMemcpyAsync(out->esc, co.esc, (size_t)esc_inline * sizeof(rafting_cesc_out_t), cudaMemcpyDeviceToHost, H->s_d2h));
         }
     }
+    if (due) CU(cudaMemcpyAsync(S.chout.p + 256, act.gids + due->n_host, (size_t)due->cap * 4, cudaMemcpyDeviceToHost, H->s_d2h));
     CU(cudaEventRecord(S.ev_done, H->s_d2h));
     S.compact_step = true; S.c_host = *out; S.c_counts_pinned = counts_land; S.c_esc_dev = co.esc;
+    S.c_tail_user = due ? due->tail_out : nullptr; S.c_tail_n = due ? due->cap : 0;
     S.dev_out = rafting_outbox_t(); memset(&S.dev_out, 0, sizeof(S.dev_out));
     S.dev_out.rep_meta = dov.rep_meta; S.dev_out.rep_term = dov.rep_term; S.dev_out.plan_meta = dov.plan_meta;
     S.dev_out.plan_pp = (rafting_i64x2_t*)dov.plan_pp; S.dev_out.plan_lc = (rafting_i64x2_t*)dov.plan_lc; S.dev_out.plan_epoch = dov.plan_epoch;
@@ -670,6 +703,23 @@ extern "C" int rafting_step_begin_compact_sweep(rafting_engine_t* e, uint32_t sl
     return compact_begin(e, slot, in, reqs, out, flags, n_active, gids, sweep);
 }
 
+// A sweep step over gids[0 .. n_host) followed by cap gids chosen on the device: the groups outside gids that the sweep
+// fires, lowest first, then groups that are not due (fillers)
+extern "C" int rafting_step_begin_compact_due(rafting_engine_t* e, uint32_t slot, uint32_t n_host, const uint32_t* gids, uint32_t cap,
+                                              const int64_t* sweep, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
+                                              const rafting_coutbox_t* out, uint32_t* tail_out, uint32_t flags) {
+    if (!e || !in || !sweep || !tail_out || (n_host && !gids)) return fail(RAFTING_E_INVAL, "bad argument");
+    if (cap == 0) return fail(RAFTING_E_INVAL, "a due step's tail holds at least one group (cap >= 1)");
+    if ((uint64_t)n_host + cap > e->G)
+        return fail(RAFTING_E_CAPACITY, "n_host %u + cap %u > max_groups %u: not enough groups outside the list to fill the tail", n_host, cap, e->G);
+    if (n_host) { if (int rc = check_active_list(e, n_host, gids)) return rc; }
+    bool has_sweep = false;
+    for (uint32_t r = 0; r < in->rows && r < e->cfg.max_rows; r++) has_sweep |= sweep[r] != 0;
+    if (!has_sweep) return fail(RAFTING_E_INVAL, "a due step needs a sweep row");
+    const DueTail due = {n_host, cap, tail_out};
+    return compact_begin(e, slot, in, reqs, out, flags, n_host + cap, gids, sweep, &due);
+}
+
 extern "C" int rafting_step_wait_compact(rafting_engine_t* e, uint32_t slot) {
     if (!e || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
     CU(cudaSetDevice(e->cfg.device));
@@ -679,6 +729,7 @@ extern "C" int rafting_step_wait_compact(rafting_engine_t* e, uint32_t slot) {
     CU(cudaEventSynchronize(S.ev_done));
     S.inflight = false;
     if (S.c_counts_pinned != S.c_host.counts) for (int k = 0; k < 4; k++) S.c_host.counts[k] = S.c_counts_pinned[k];
+    if (S.c_tail_user) { memcpy(S.c_tail_user, S.chout.p + 256, (size_t)S.c_tail_n * 4); S.c_tail_user = nullptr; }
     const uint32_t n = S.c_counts_pinned[0] < S.c_host.esc_cap ? S.c_counts_pinned[0] : S.c_host.esc_cap;
     if (n > CESC_INLINE) {                                                    // rare: more than the records that travelled with the columns
         CU(cudaMemcpyAsync(S.c_host.esc + CESC_INLINE, (const rafting_cesc_out_t*)S.c_esc_dev + CESC_INLINE,

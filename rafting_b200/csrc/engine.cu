@@ -470,6 +470,8 @@ struct Slot {
     Blk creq, creqw;                          // compact path: request list + entry pool, and its scan scratch
     bool compact_step = false;                // the step in flight came through rafting_step_begin_compact[_req]
     rafting_coutbox_t c_host; size_t c_esc_off = 0; uint32_t* c_counts_pinned = nullptr; void* c_esc_dev = nullptr;
+    Blk ctail;                                // rafting_step_begin_compact_due: the tail selection's scratch (timers.cuh)
+    uint32_t* c_tail_user = nullptr; uint32_t c_tail_n = 0;   // where the wait copies the tail (landed at chout + 256)
     Blk hin, hout;                            // pinned host staging (leases only), same layout as din / dout
     uint32_t* h_flags = nullptr;              // pinned landing place of the flag words on the caller-owned path
     cudaEvent_t ev_h2d = nullptr, ev_kernel = nullptr, ev_done = nullptr;
@@ -525,6 +527,7 @@ static void hostpath_free(rafting_engine* e) {
         if (s.chout.p) cudaFreeHost(s.chout.p);
         if (s.creq.p) cudaFree(s.creq.p);
         if (s.creqw.p) cudaFree(s.creqw.p);
+        if (s.ctail.p) cudaFree(s.ctail.p);
         if (s.ev_h2d) cudaEventDestroy(s.ev_h2d);
         if (s.ev_kernel) cudaEventDestroy(s.ev_kernel);
         if (s.ev_done) cudaEventDestroy(s.ev_done);

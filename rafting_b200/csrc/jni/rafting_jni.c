@@ -134,6 +134,15 @@ JNIEXPORT void JNICALL FN(stepBeginCompactSweep)(JNIEnv* env, jclass k, jlong h,
                                            (const rafting_cinbox_t*)BUF(cin), (const rafting_creqs_t*)BUF(creqs), (const rafting_coutbox_t*)BUF(cout),
                                            (uint32_t)flags));
 }
+/* ... over nHost listed gids (null when nHost = 0) and a tail of cap gids chosen on the device: every column of cinbox /
+   coutbox sized by nHost + cap; tailOut (cap uint32, direct) receives the tail at stepWaitCompact, coutbox counts[3] the
+   number of due groups outside the list */
+JNIEXPORT void JNICALL FN(stepBeginCompactDue)(JNIEnv* env, jclass k, jlong h, jint slot, jint nHost, jobject gids, jint cap, jobject sweep,
+                                               jobject cin, jobject creqs, jobject cout, jobject tailOut, jint flags) {
+    CHECK(rafting_step_begin_compact_due(ENG(h), (uint32_t)slot, (uint32_t)nHost, (const uint32_t*)BUF(gids), (uint32_t)cap,
+                                         (const int64_t*)BUF(sweep), (const rafting_cinbox_t*)BUF(cin), (const rafting_creqs_t*)BUF(creqs),
+                                         (const rafting_coutbox_t*)BUF(cout), (uint32_t*)BUF(tailOut), (uint32_t)flags));
+}
 JNIEXPORT void JNICALL FN(stepWaitCompact)(JNIEnv* env, jclass k, jlong h, jint slot) { CHECK(rafting_step_wait_compact(ENG(h), (uint32_t)slot)); }
 /* the groups a sweep at untilMs would fire: gidsOut (cap uint32) is filled at the wait; result = {nDue, nextDeadlineMs} */
 JNIEXPORT void JNICALL FN(timersDueBegin)(JNIEnv* env, jclass k, jlong h, jint slot, jlong untilMs, jobject gidsOut, jint cap) {

@@ -85,7 +85,121 @@ __global__ void __launch_bounds__(DUE_TPB) due_emit_kernel(const uint32_t* __res
     }
 }
 
+// ---- the tail of a step begun with rafting_step_begin_compact_due ----
+// The step's list is the host's gids (positions 0 .. n_host) followed by a tail of cap gids chosen on the step stream, after
+// the slot's H2D copy and before unpack_kernel, so the choice sees the state the step itself will see:
+//   tail_member_kernel   one thread per host position sets its gid's bit in a G-bit mask (zeroed by a memset before it)
+//   tail_scan_kernel     one thread per group, due_scan_kernel's predicate: a due-unlisted and an idle-unlisted bit go into two
+//                        warp masks, and each block leaves its two counts packed in one word, due << 32 | idle, so that one
+//                        cub::DeviceScan sum carries both (each count stays below 2^32: no carry crosses)
+//   tail_emit_kernel     due gids from tail position 0, then idle ones (fillers) from min(due total, cap), both in increasing
+//                        order, stopping at cap; one thread writes the due total (counts[3])
+// Fillers keep the step's n host-known, so unpack / step / pack run unchanged over the device-written gids column: a listed
+// group with no event whose timer is not due is left untouched by a sweep row.  DueAgg does not fit here (two counts, no
+// deadline), hence the packed sum.
+constexpr uint32_t TAIL_WARPS = DUE_TPB / 32;
+
+__global__ void tail_member_kernel(const uint32_t* __restrict__ gids, uint32_t n_host, uint32_t* __restrict__ member) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n_host) { const uint32_t g = gids[k]; atomicOr(member + (g >> 5), 1u << (g & 31u)); }
+}
+
+__global__ void __launch_bounds__(DUE_TPB) tail_scan_kernel(Tables T, int64_t until, const uint32_t* __restrict__ member,
+                                                            uint32_t* __restrict__ mask, uint64_t* __restrict__ agg) {
+    __shared__ uint32_t wdue[TAIL_WARPS], widle[TAIL_WARPS];
+    const uint32_t g = blockIdx.x * DUE_TPB + threadIdx.x;
+    bool due = false, idle = false;
+    if (g < T.G) {
+        const uint32_t w = (uint32_t)T.g_meta[g];
+        const int64_t timer = T.g_timer[g];
+        const bool alive = (w & W_ALIVE) != 0, leader = (w & W_ROLE_MASK) == RAFTING_ROLE_LEADER;
+        const bool armed = alive && (leader || (timer > 0 && timer != I64MAX));
+        const bool listed = (member[g >> 5] >> (g & 31u)) & 1u;
+        due = !listed && armed && timer <= until;
+        idle = !listed && !due;
+    }
+    const uint32_t lane = threadIdx.x & 31u, wq = threadIdx.x >> 5;
+    const uint32_t md = __ballot_sync(0xffffffffu, due), mi = __ballot_sync(0xffffffffu, idle);
+    if (lane == 0) {
+        const size_t at = ((size_t)blockIdx.x * TAIL_WARPS + wq) * 2;
+        mask[at] = md; mask[at + 1] = mi; wdue[wq] = __popc(md); widle[wq] = __popc(mi);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint64_t d = 0, i = 0;
+        for (uint32_t k = 0; k < TAIL_WARPS; k++) { d += wdue[k]; i += widle[k]; }
+        agg[blockIdx.x] = (d << 32) | i;
+    }
+}
+
+__global__ void __launch_bounds__(DUE_TPB) tail_emit_kernel(const uint32_t* __restrict__ mask, const uint64_t* __restrict__ agg,
+                                                            const uint64_t* __restrict__ off, uint32_t nblocks,
+                                                            uint32_t* __restrict__ tail, uint32_t cap, uint32_t* __restrict__ n_due) {
+    __shared__ uint32_t bdue[TAIL_WARPS], bidle[TAIL_WARPS];
+    const uint64_t total = off[nblocks - 1] + agg[nblocks - 1];
+    const uint32_t due_total = (uint32_t)(total >> 32), first_filler = due_total < cap ? due_total : cap;
+    if (blockIdx.x == 0 && threadIdx.x == 0) *n_due = due_total;
+    const uint64_t o = off[blockIdx.x];
+    const uint32_t od = (uint32_t)(o >> 32), oi = (uint32_t)o;
+    if (od >= cap && (uint64_t)first_filler + oi >= cap) return;          // every entry of this block lies past the tail
+    const uint32_t* bm = mask + (size_t)blockIdx.x * TAIL_WARPS * 2;
+    if (threadIdx.x == 0) {
+        uint32_t d = od, i = oi;
+        for (uint32_t k = 0; k < TAIL_WARPS; k++) { bdue[k] = d; bidle[k] = i; d += __popc(bm[2 * k]); i += __popc(bm[2 * k + 1]); }
+    }
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31u, wq = threadIdx.x >> 5, below = (1u << lane) - 1u;
+    const uint32_t md = bm[2 * wq], mi = bm[2 * wq + 1];
+    const uint32_t g = blockIdx.x * DUE_TPB + threadIdx.x;
+    if ((md >> lane) & 1u) {
+        const uint32_t pos = bdue[wq] + __popc(md & below);
+        if (pos < cap) tail[pos] = g;
+    } else if ((mi >> lane) & 1u) {
+        const uint64_t pos = (uint64_t)first_filler + bidle[wq] + __popc(mi & below);
+        if (pos < cap) tail[pos] = g;
+    }
+}
+
 }  // namespace rafting
+
+// device scratch of one tail selection over G groups: member mask, warp masks, block counts, their scan, CUB's scratch
+struct TailLayout { size_t member, mask, agg, off, tmp, total; uint32_t nblocks; };
+static int tail_layout(uint32_t G, TailLayout& L) {
+    using namespace rafting;
+    L.nblocks = (G + DUE_TPB - 1) / DUE_TPB;
+    size_t scan_tmp = 0;
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)L.nblocks));
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; };
+    L.member = take((size_t)L.nblocks * TAIL_WARPS * 4); L.mask = take((size_t)L.nblocks * TAIL_WARPS * 8);
+    L.agg = take((size_t)L.nblocks * 8); L.off = take((size_t)L.nblocks * 8); L.tmp = take(scan_tmp);
+    L.total = o;
+    return RAFTING_OK;
+}
+static int tail_scratch_bytes(uint32_t G, size_t* bytes) {
+    TailLayout L;
+    if (int rc = tail_layout(G, L)) return rc;
+    *bytes = L.total;
+    return RAFTING_OK;
+}
+
+// Enqueues the tail selection on the engine's stream: list[0 .. n_host) is the host's part (device copy), the tail goes to
+// list[n_host .. n_host + cap), the due total to *n_due.  scratch holds tail_layout(G).total bytes.
+static int tail_select(rafting_engine* e, uint8_t* scratch, int64_t until, uint32_t* list, uint32_t n_host, uint32_t cap, uint32_t* n_due) {
+    using namespace rafting;
+    TailLayout L;
+    if (int rc = tail_layout(e->G, L)) return rc;
+    uint32_t* member = (uint32_t*)(scratch + L.member); uint32_t* mask = (uint32_t*)(scratch + L.mask);
+    uint64_t* agg = (uint64_t*)(scratch + L.agg); uint64_t* off = (uint64_t*)(scratch + L.off);
+    CU(cudaMemsetAsync(member, 0, (size_t)L.nblocks * TAIL_WARPS * 4, e->stream));
+    if (n_host) tail_member_kernel<<<(n_host + 255u) / 256u, 256, 0, e->stream>>>(list, n_host, member);
+    tail_scan_kernel<<<L.nblocks, DUE_TPB, 0, e->stream>>>(e->T, until, member, mask, agg);
+    size_t tb = L.total - L.tmp;
+    CU(cub::DeviceScan::ExclusiveSum(scratch + L.tmp, tb, agg, off, (int)L.nblocks, e->stream));
+    tail_emit_kernel<<<L.nblocks, DUE_TPB, 0, e->stream>>>(mask, agg, off, L.nblocks, list + n_host, cap, n_due);
+    CU(cudaGetLastError());
+    return RAFTING_OK;
+}
 
 // One query slot: device scratch, a mapped pinned block for the result (and the list when the caller's buffer is not mapped)
 struct DueSlot {

@@ -38,7 +38,7 @@ EXPORTS = [
     "rafting_comm_init", "rafting_comm_init_all", "rafting_comm_unique_id", "rafting_allgather_commit", "rafting_allgather_commit_from",
     "rafting_allgather_commit_all", "rafting_allgather_last", "rafting_restore_async", "rafting_state_save", "rafting_state_load", "rafting_step_device_seq", "rafting_engine_stream",
     "rafting_engine_counters", "rafting_abi_sizes", "rafting_checkpoint", "rafting_restore",
-    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_step_begin_compact_active", "rafting_step_begin_compact_sweep", "rafting_timers_due_begin", "rafting_timers_due_wait", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
+    "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_step_begin_compact_active", "rafting_step_begin_compact_sweep", "rafting_step_begin_compact_due", "rafting_timers_due_begin", "rafting_timers_due_wait", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
     "rafting_log_config", "rafting_log_append", "rafting_log_read", "rafting_log_gather", "rafting_log_trim", "rafting_log_stats",
     "rafting_log_store_open", "rafting_log_sync", "rafting_log_mark", "rafting_log_recovered", "rafting_log_export_kv", "rafting_log_store_stats",
 ]
@@ -121,6 +121,9 @@ def lib():
                                                         C.POINTER(abi.CReqsC), C.POINTER(abi.COutboxC), C.c_uint32]
         L.rafting_step_begin_compact_sweep.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(abi.CInboxC),
                                                        C.POINTER(abi.CReqsC), C.POINTER(abi.COutboxC), C.c_uint32]
+        L.rafting_step_begin_compact_due.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
+                                                     C.POINTER(abi.CInboxC), C.POINTER(abi.CReqsC), C.POINTER(abi.COutboxC),
+                                                     C.c_void_p, C.c_uint32]
         L.rafting_timers_due_begin.argtypes = [C.c_void_p, C.c_uint32, C.c_int64, C.c_void_p, C.c_uint32]
         L.rafting_timers_due_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_int64)]
         L.rafting_compact_req_layout.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64 * 4)]
@@ -278,6 +281,42 @@ class Engine:
         _check(lib().rafting_step_begin_compact_sweep(self._h, slot, n, g, sweep.ctypes.data, C.byref(cin_c),
                                                       None if reqs_c is None else C.byref(reqs_c), C.byref(cout_c), flags),
                "rafting_step_begin_compact_sweep")
+
+    def step_begin_compact_due(self, slot: int, gids: np.ndarray, cap: int, sweep: np.ndarray, cin_c: abi.CInboxC,
+                               reqs_c: abi.CReqsC | None, cout_c: abi.COutboxC, flags: int = 0):
+        """rafting_step_begin_compact_due: a sweep step over gids (uint32, strictly increasing, may be empty) followed by a tail
+        of cap gids the device chooses (the groups outside gids that the sweep fires, lowest first, then groups that are not
+        due).  Every column of cin_c / cout_c holds len(gids) + cap groups per row, by position; counts[3] of the outbox is the
+        number of due groups outside gids.  gids and sweep must stay alive until step_wait_compact_due, which returns the tail."""
+        if gids.dtype != np.uint32 or not gids.flags.c_contiguous:
+            raise TypeError("gids must be a contiguous uint32 array")
+        if sweep.dtype != np.int64 or not sweep.flags.c_contiguous:
+            raise TypeError("sweep must be a contiguous int64 array")
+        if len(sweep) < cin_c.rows:
+            raise ValueError(f"sweep holds {len(sweep)} rows, the inbox {cin_c.rows}")
+        if cap < 1:
+            raise ValueError("cap must be at least 1")
+        tail = np.zeros(cap, dtype=np.uint32)
+        _check(lib().rafting_step_begin_compact_due(self._h, slot, len(gids), gids.ctypes.data if len(gids) else None, cap,
+                                                    sweep.ctypes.data, C.byref(cin_c), None if reqs_c is None else C.byref(reqs_c),
+                                                    C.byref(cout_c), tail.ctypes.data, flags), "rafting_step_begin_compact_due")
+        self._due_tail = getattr(self, "_due_tail", {})
+        self._due_tail[slot] = tail
+
+    def step_wait_compact_due(self, slot: int) -> np.ndarray:
+        """rafting_step_wait_compact for a step begun with step_begin_compact_due: -> its tail (uint32 [cap])."""
+        self.step_wait_compact(slot)
+        return self._due_tail.pop(slot)
+
+    def step_compact_due(self, cin, cout, cap: int, slot: int = 0, reqs=None, flags: int = 0) -> np.ndarray:
+        """Synchronous due step: cin a compact.CompactInbox encoded with sweep=True over cin.gids (the host's part, which may
+        be empty) padded with cap empty positions (compact.pad_for_tail), cout a CompactOutbox of len(cin.gids) + cap groups.
+        On return cout.gids is the whole list, gids followed by the tail; returns the tail."""
+        host = cin.gids if cin.gids is not None else np.zeros(0, np.uint32)
+        self.step_begin_compact_due(slot, host, cap, cin.sweep, cin.as_c(), None if reqs is None else reqs.as_c(), cout.as_c(), flags)
+        tail = self.step_wait_compact_due(slot)
+        cout.gids = np.concatenate([host, tail]).astype(np.uint32)
+        return tail
 
     def timers_due_begin(self, slot: int, until_ms: int, out: np.ndarray | int | None, cap: int | None = None):
         """rafting_timers_due_begin: enqueue the query "which groups would a sweep at until_ms fire" behind every step begun

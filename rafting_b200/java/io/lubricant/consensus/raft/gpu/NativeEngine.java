@@ -33,6 +33,7 @@ final class NativeEngine {
     static native void stepBeginCompactEx(long h, int slot, ByteBuffer cinbox, ByteBuffer creqs, ByteBuffer coutbox, int flags);   // rafting_step_begin_compact_ex: RAFTING_COMPACT_ELECTIONS
     static native void stepBeginCompactActive(long h, int slot, int nActive, ByteBuffer gids, ByteBuffer cinbox, ByteBuffer creqs, ByteBuffer coutbox, int flags);   // rafting_step_begin_compact_active: over an active list
     static native void stepBeginCompactSweep(long h, int slot, int nActive, ByteBuffer gids, ByteBuffer sweep, ByteBuffer cinbox, ByteBuffer creqs, ByteBuffer coutbox, int flags);   // rafting_step_begin_compact_sweep: with sweep rows (timers)
+    static native void stepBeginCompactDue(long h, int slot, int nHost, ByteBuffer gids, int cap, ByteBuffer sweep, ByteBuffer cinbox, ByteBuffer creqs, ByteBuffer coutbox, ByteBuffer tailOut, int flags);   // rafting_step_begin_compact_due: the device lists the due groups
     static native void timersDueBegin(long h, int slot, long untilMs, ByteBuffer gidsOut, int cap);   // rafting_timers_due_begin: the groups a sweep would fire
     static native void timersDueWait(long h, int slot, long[] nDueAndNextDeadline);              // rafting_timers_due_wait
     static native void stepWaitCompact(long h, int slot);                                        // rafting_step_wait_compact
