@@ -338,6 +338,14 @@ __global__ void __launch_bounds__(256) pack_kernel(Tables T, uint32_t rows, Outb
     }
 }
 
+// the kernel variants of a step: unpack [EL][AL], pack [EL][PT][AL], unpack_requests [EL]
+static const decltype(&unpack_kernel<false, false>) UNPACK[2][2] = {
+    {unpack_kernel<false, false>, unpack_kernel<false, true>}, {unpack_kernel<true, false>, unpack_kernel<true, true>}};
+static const decltype(&pack_kernel<false, false, false>) PACK[2][2][2] = {
+    {{pack_kernel<false, false, false>, pack_kernel<false, false, true>}, {pack_kernel<false, true, false>, pack_kernel<false, true, true>}},
+    {{pack_kernel<true, false, false>, pack_kernel<true, false, true>}, {pack_kernel<true, true, false>, pack_kernel<true, true, true>}}};
+static const decltype(&unpack_requests_kernel<false>) UNPACK_REQUESTS[2] = {unpack_requests_kernel<false>, unpack_requests_kernel<true>};
+
 }  // namespace rafting
 
 struct CompactState {
@@ -361,20 +369,18 @@ static int compact_state(rafting_engine* e) {
 }
 
 // byte layout of the two wire blocks of a slot (device copy and — for the small items — a pinned landing block)
-struct CLayout { size_t row_base, op_c, op_un, ev_c, esc, in_total; size_t plan_c, rep_c, commit, term, role, inc, err, last, epoch, counts, esc_out, out_total, out_dense; };
+struct CLayout { size_t row_base, op_c, op_un, ev_c, esc, in_total; size_t plan_c, rep_c, commit, term, role, inc, err, last, epoch, counts, esc_out, out_total; };
 static CLayout compact_layout(size_t rows, size_t G, size_t F, size_t n_esc_in, size_t esc_cap) {
-    CLayout L; size_t o = 0;
-    auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; };
+    CLayout L; Carve in, out;
     // the optional parts come last, so that the single copy of a block-shaped inbox ends where the launch's data ends
-    L.row_base = take(rows * 8); L.op_c = take(rows * G * 4); L.ev_c = take(rows * G * F * 4); L.op_un = take(rows * G * 2);
-    L.esc = take((n_esc_in + 1) * sizeof(rafting_cesc_in_t));
-    L.in_total = o; o = 0;
-    L.plan_c = take(rows * G * F * 4); L.rep_c = take(rows * G);
-    L.commit = take(G * 8); L.term = take(G * 8); L.role = take(G * 4); L.inc = take(G * 4); L.err = take(G * 4); L.last = take(G * 16); L.epoch = take(G * 16);
-    L.counts = take(16);
-    L.out_dense = o;                                                          // everything before the escape list travels down every step
-    L.esc_out = take((esc_cap + 1) * sizeof(rafting_cesc_out_t));
-    L.out_total = o;
+    L.row_base = in.take(rows * 8); L.op_c = in.take(rows * G * 4); L.ev_c = in.take(rows * G * F * 4); L.op_un = in.take(rows * G * 2);
+    L.esc = in.take((n_esc_in + 1) * sizeof(rafting_cesc_in_t));
+    L.in_total = in.o;
+    L.plan_c = out.take(rows * G * F * 4); L.rep_c = out.take(rows * G);
+    L.commit = out.take(G * 8); L.term = out.take(G * 8); L.role = out.take(G * 4); L.inc = out.take(G * 4); L.err = out.take(G * 4); L.last = out.take(G * 16); L.epoch = out.take(G * 16);
+    L.counts = out.take(16);
+    L.esc_out = out.take((esc_cap + 1) * sizeof(rafting_cesc_out_t));
+    L.out_total = out.o;
     return L;
 }
 
@@ -396,16 +402,43 @@ extern "C" int rafting_compact_layout(uint32_t rows, uint32_t G, uint32_t F, uin
 // the request list's block: records, op escapes, then the entry pool (the device block extends the pool by the records' terms)
 struct CRLayout { size_t req, esc, ent, total; };
 static CRLayout compact_req_layout(size_t n_req, size_t n_esc, size_t ent_count) {
-    CRLayout L; size_t o = 0;
-    auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; };
-    L.req = take(n_req * sizeof(rafting_creq_t)); L.esc = take(n_esc * sizeof(rafting_cesc_op_t)); L.ent = o; o += ent_count * 8;
-    L.total = o;
+    CRLayout L; Carve c;
+    L.req = c.take(n_req * sizeof(rafting_creq_t)); L.esc = c.take(n_esc * sizeof(rafting_cesc_op_t)); L.ent = c.o;
+    L.total = L.ent + ent_count * 8;
     return L;
 }
 extern "C" int rafting_compact_req_layout(uint32_t n_req, uint32_t n_op_esc, uint32_t ent_count, uint64_t off[4]) {
     if (!off) return fail(RAFTING_E_INVAL, "null argument");
     const CRLayout L = compact_req_layout(n_req, n_op_esc, ent_count);
     off[0] = L.req; off[1] = L.esc; off[2] = L.ent; off[3] = L.total;
+    return RAFTING_OK;
+}
+
+// One column of a wire block: the caller's memory (absent when null or bytes == 0) and its offset in the engine's layout
+struct WireCol { const void* h; size_t at, bytes; };
+// The caller's block, or null: a caller that carved its columns from one block with the layout above has every present
+// column at its laid-out offset from one base
+static uint8_t* wire_block(const WireCol* c, int n) {
+    uint8_t* base = nullptr;
+    for (int k = 0; k < n; k++) {
+        if (!c[k].h || !c[k].bytes) continue;
+        uint8_t* b = (uint8_t*)c[k].h - c[k].at;
+        if (!base) base = b;
+        else if (b != base) return nullptr;
+    }
+    return base;
+}
+// Between the caller's columns and the device block dev: ONE copy of the caller's block hb up to the end of its last present
+// column, or (hb null) one copy per present column
+static int wire_copy(const WireCol* c, int n, uint8_t* hb, uint8_t* dev, cudaMemcpyKind dir, cudaStream_t st) {
+    const bool up = dir == cudaMemcpyHostToDevice;
+    size_t end = 0;
+    for (int k = 0; k < n; k++) {
+        if (!c[k].h || !c[k].bytes) continue;
+        end = c[k].at + c[k].bytes > end ? c[k].at + c[k].bytes : end;
+        if (!hb) CU(cudaMemcpyAsync(up ? dev + c[k].at : (void*)c[k].h, up ? c[k].h : dev + c[k].at, c[k].bytes, dir, st));
+    }
+    if (hb) CU(cudaMemcpyAsync(up ? (void*)dev : hb, up ? hb : dev, end, dir, st));
     return RAFTING_OK;
 }
 
@@ -420,25 +453,52 @@ extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot
 
 // the device-chosen tail of a step begun with rafting_step_begin_compact_due (timers.cuh)
 struct DueTail { uint32_t n_host, cap; uint32_t* tail_out; };
-static int tail_scratch_bytes(uint32_t G, size_t* bytes);
+static int tail_reserve(rafting_engine* e, Blk& scratch);
 static int tail_select(rafting_engine* e, uint8_t* scratch, int64_t until, uint32_t* list, uint32_t n_host, uint32_t cap, uint32_t* n_due);
 
-// One compact step in `slot`: over the whole shard (gids == nullptr, n = G), or over the n groups gids[0 .. n) that the caller
-// has checked (strictly increasing, each < G).  Every wire column and every dense staging column holds n groups per row.
-// sweep (host, [rows], may be null): the step's row_now column (rafting_step_begin_compact_sweep).
-// due (rafting_step_begin_compact_due): gids holds due->n_host entries and n_active = n_host + cap; the device writes the
-// rest of the list before unpack_kernel reads it.
-static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
-                         const rafting_coutbox_t* out, uint32_t flags, uint32_t n_active, const uint32_t* gids,
-                         const int64_t* sweep = nullptr, const DueTail* due = nullptr) {
-    using namespace rafting;
-    if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
+// The list is checked in full before anything is enqueued: a lane's tag bitmap must have exactly one owning thread, and the
+// in-flight table is indexed by gid, so a duplicate or an id past max_groups would race on it or index past it.
+static int check_active_list(rafting_engine_t* e, uint32_t n_active, const uint32_t* gids) {
+    if (!e || !gids) return fail(RAFTING_E_INVAL, "bad argument");
+    if (n_active == 0) return fail(RAFTING_E_INVAL, "an active list holds at least one group");
+    if (n_active > e->G) return fail(RAFTING_E_CAPACITY, "n_active %u > max_groups %u", n_active, e->G);
+    for (uint32_t k = 0; k < n_active; k++) {
+        if (gids[k] >= e->G) return fail(RAFTING_E_INVAL, "gids[%u] = %u is not below max_groups", k, gids[k]);
+        if (k > 0 && gids[k] <= gids[k - 1]) return fail(RAFTING_E_INVAL, "gids must be strictly increasing (gids[%u] = %u)", k, gids[k]);
+    }
+    return RAFTING_OK;
+}
+
+// One compact step: its arguments, what compact_check found, and the slot's blocks and staging views compact_reserve made
+struct CompactStep {
+    const rafting_cinbox_t* in; const rafting_creqs_t* reqs; const rafting_coutbox_t* out;
+    const uint32_t* gids; const int64_t* sweep; const DueTail* due;
+    size_t rows, n, n_listed;                    // n: groups per row of the step; n_listed: entries of gids the host wrote
+    bool list, has_reqs, has_sweep, el, pt;
+    size_t n_req, n_oesc, ent_esc, pool;         // records, op escapes, entries the host sends, the step's entry pool
+    Layout LD; CLayout LC; CRLayout LR;          // dense staging, wire blocks, request block
+    size_t w_counts, w_offs, w_tmp, scan_tmp;    // the request scan's scratch (S.creqw): order word, counts, offsets, CUB's
+    size_t sweep_at;                             // offset of the sweep column in the staged copy of [gids | pad] sweep
+    rafting_inbox_t din; rafting_outbox_t dout;  // the dense staging views the step kernel works on
+};
+
+// Every refusal of a compact step, before anything is enqueued (the slot stays free); fills the step's shape into p
+static int compact_check(rafting_engine_t* e, uint32_t slot, uint32_t flags, uint32_t n_active, CompactStep& p) {
+    const rafting_cinbox_t* in = p.in; const rafting_creqs_t* reqs = p.reqs; const rafting_coutbox_t* out = p.out; const DueTail* due = p.due;
+    if (!e || !in || !out || slot >= RAFTING_HOST_SLOTS || (due && (!p.sweep || !due->tail_out || (due->n_host && !p.gids))))
+        return fail(RAFTING_E_INVAL, "bad argument");
+    if (p.sweep) for (uint32_t r = 0; r < in->rows && r < e->cfg.max_rows; r++) p.has_sweep |= p.sweep[r] != 0;
+    if (due) {
+        if (due->cap == 0) return fail(RAFTING_E_INVAL, "a due step's tail holds at least one group (cap >= 1)");
+        if ((uint64_t)due->n_host + due->cap > e->G)
+            return fail(RAFTING_E_CAPACITY, "n_host %u + cap %u > max_groups %u: not enough groups outside the list to fill the tail", due->n_host, due->cap, e->G);
+        if (due->n_host) { if (int rc = check_active_list(e, due->n_host, p.gids)) return rc; }
+        if (!p.has_sweep) return fail(RAFTING_E_INVAL, "a due step needs a sweep row");
+    }
     if (flags & ~(RAFTING_COMPACT_ELECTIONS | RAFTING_COMPACT_PREV_TERM)) return fail(RAFTING_E_INVAL, "unknown compact step flags 0x%x", flags);
-    const bool el = (flags & RAFTING_COMPACT_ELECTIONS) != 0, pt = (flags & RAFTING_COMPACT_PREV_TERM) != 0;
-    const bool has_reqs = reqs && (reqs->n_req || reqs->n_op_esc);
-    bool has_sweep = false;
-    if (sweep) for (uint32_t r = 0; r < in->rows && r < e->cfg.max_rows; r++) has_sweep |= sweep[r] != 0;
-    if (!in->row_base || (!in->op_c && !in->ev_c && !has_reqs && !has_sweep))
+    p.el = (flags & RAFTING_COMPACT_ELECTIONS) != 0; p.pt = (flags & RAFTING_COMPACT_PREV_TERM) != 0;
+    p.has_reqs = reqs && (reqs->n_req || reqs->n_op_esc);
+    if (!in->row_base || (!in->op_c && !in->ev_c && !p.has_reqs && !p.has_sweep))
         return fail(RAFTING_E_INVAL, "compact inbox needs row_base and at least one of op_c / ev_c / a request / a sweep row");
     if (reqs && ((reqs->n_req && !reqs->req) || (reqs->n_op_esc && !reqs->op_esc) || (reqs->ent_count && !reqs->ent_terms)))
         return fail(RAFTING_E_INVAL, "request list: a count without its array");
@@ -453,219 +513,182 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     CU(cudaSetDevice(e->cfg.device));
     int rc = hostpath_init(e); if (rc) return rc;
     if ((rc = compact_state(e))) return rc;
-    HostPath* H = hp(e); Slot& S = H->slot[slot];
+    const Slot& S = hp(e)->slot[slot];
     if (S.leased) return fail(RAFTING_E_BUSY, "slot %u is held by an outstanding lease", slot);
     if (S.inflight) return fail(RAFTING_E_BUSY, "slot %u has a step in flight", slot);
-    const bool list = gids != nullptr || due != nullptr;
-    const size_t rows = in->rows, n = list ? n_active : e->G, F = e->F;       // n: groups per row of the step
-    const size_t n_listed = due ? due->n_host : n;                            // entries of gids the host wrote
+    p.list = p.gids != nullptr || due != nullptr;
+    const size_t rows = in->rows, n = p.list ? n_active : e->G, F = e->F;
+    p.rows = rows; p.n = n; p.n_listed = due ? due->n_host : n;
     if (rows == 0 || rows > e->cfg.max_rows) return fail(RAFTING_E_CAPACITY, "rows %zu beyond max_rows %u", rows, e->cfg.max_rows);
-    const size_t n_req = has_reqs ? reqs->n_req : 0, n_oesc = has_reqs ? reqs->n_op_esc : 0;
-    if (has_reqs && (uint64_t)rows * n * F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
-    if (n_req > rows * n || n_oesc > rows * n || n_req > 0x7fffffffu)
+    p.n_req = p.has_reqs ? reqs->n_req : 0; p.n_oesc = p.has_reqs ? reqs->n_op_esc : 0;
+    if (p.has_reqs && (uint64_t)rows * n * F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
+    if (p.n_req > rows * n || p.n_oesc > rows * n || p.n_req > 0x7fffffffu)
         return fail(RAFTING_E_INVAL, "a request list longer than rows * n cannot be strictly increasing");
-    if (has_sweep) {
-        // a sweep row's op slot belongs to the sweep: the step would drop a request placed there without a trace
-        for (size_t k = 0; k < n_req + n_oesc; k++) {
-            const uint32_t at = k < n_req ? reqs->req[k].slot : reqs->op_esc[k - n_req].slot;
-            if (at < rows * n && sweep[at / n] != 0)
-                return fail(RAFTING_E_INVAL, "%s %zu (slot %u) lies on sweep row %zu", k < n_req ? "request record" : "op escape",
-                            k < n_req ? k : k - n_req, at, (size_t)(at / n));
-        }
+    // A sweep row's op slot belongs to the sweep: the step would drop a request placed there without a trace.  A due step
+    // (always with a sweep row) chooses its tail's groups on the device: nothing the host sends can name one of their positions.
+    for (size_t k = 0; p.has_sweep && k < p.n_req + p.n_oesc; k++) {
+        const uint32_t at = k < p.n_req ? reqs->req[k].slot : reqs->op_esc[k - p.n_req].slot;
+        const char* what = k < p.n_req ? "request record" : "op escape";
+        const size_t j = k < p.n_req ? k : k - p.n_req;
+        if (at < rows * n && p.sweep[at / n] != 0) return fail(RAFTING_E_INVAL, "%s %zu (slot %u) lies on sweep row %zu", what, j, at, (size_t)(at / n));
+        if (at < rows * n && due && at % n >= p.n_listed) return fail(RAFTING_E_INVAL, "%s %zu (slot %u) lies at tail position %zu", what, j, at, (size_t)(at % n));
     }
-    if (due) {
-        // the tail's groups are chosen on the device: nothing the host sends can name one of its positions
-        for (size_t k = 0; k < n_req + n_oesc; k++) {
-            const uint32_t at = k < n_req ? reqs->req[k].slot : reqs->op_esc[k - n_req].slot;
-            if (at < rows * n && at % n >= n_listed)
-                return fail(RAFTING_E_INVAL, "%s %zu (slot %u) lies at tail position %zu", k < n_req ? "request record" : "op escape",
-                            k < n_req ? k : k - n_req, at, (size_t)(at % n));
-        }
-        for (uint32_t k = 0; k < in->n_esc; k++) {
-            const uint32_t at = in->esc[k].slot;
-            if (at < rows * n * F && (at / F) % n >= n_listed)
-                return fail(RAFTING_E_INVAL, "escape record %u (slot %u) lies at tail position %zu", k, at, (size_t)((at / F) % n));
-        }
+    for (uint32_t k = 0; due && k < in->n_esc; k++) {
+        const uint32_t at = in->esc[k].slot;
+        if (at < rows * n * F && (at / F) % n >= p.n_listed)
+            return fail(RAFTING_E_INVAL, "escape record %u (slot %u) lies at tail position %zu", k, at, (size_t)((at / F) % n));
     }
-    const size_t ent_esc = has_reqs ? reqs->ent_count : 0, pool = has_reqs ? ent_esc + reqs->req_entries : 0;
-    // dense staging the step kernel works on (the entry pool lives in the request block); with an active list its group
-    // columns are positional (RAFTING_INBOX_COMPACT_GROUPS) and the list itself travels in its gids column
-    const Layout LD = make_layout(rows, n, F, n, list ? n : 0, 0);
-    const CLayout LC = compact_layout(rows, n, F, in->n_esc, out->esc_cap);
-    const CRLayout LR = compact_req_layout(n_req, n_oesc, ent_esc);
-    size_t scan_tmp = 0;
-    if (n_req) CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n_req));
-    const size_t w_counts = 256, w_offs = w_counts + ((n_req * 8 + 255) & ~(size_t)255), w_tmp = w_offs + ((n_req * 8 + 255) & ~(size_t)255);
-    if ((rc = blk_reserve(S.din, LD.in_total, false)) || (rc = blk_reserve(S.dout, LD.out_total, false)) ||
-        (rc = blk_reserve(S.cin, LC.in_total, false)) || (rc = blk_reserve(S.cout, LC.out_total, false)) ||
-        (rc = blk_reserve(S.chout, 256 + (due ? (size_t)due->cap * 4 : 0), true))) return rc;
-    size_t tail_bytes = 0;
-    if (due && ((rc = tail_scratch_bytes(e->G, &tail_bytes)) || (rc = blk_reserve(S.ctail, tail_bytes, false)))) return rc;
+    p.ent_esc = p.has_reqs ? reqs->ent_count : 0; p.pool = p.has_reqs ? p.ent_esc + reqs->req_entries : 0;
+    return RAFTING_OK;
+}
+
+// The slot's blocks for the step, and the dense staging views the step kernel works on
+static int compact_reserve(rafting_engine_t* e, Slot& S, CompactStep& p) {
+    const size_t rows = p.rows, n = p.n, F = e->F;
+    // the entry pool lives in the request block; with an active list the group columns are positional
+    // (RAFTING_INBOX_COMPACT_GROUPS) and the list itself travels in the gids column
+    p.LD = make_layout(rows, n, F, n, p.list ? n : 0, 0);
+    p.LC = compact_layout(rows, n, F, p.in->n_esc, p.out->esc_cap);
+    p.LR = compact_req_layout(p.n_req, p.n_oesc, p.ent_esc);
+    if (p.n_req) CU(cub::DeviceScan::ExclusiveSum(nullptr, p.scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)p.n_req));
+    Carve w; w.take(4); p.w_counts = w.take(p.n_req * 8); p.w_offs = w.take(p.n_req * 8); p.w_tmp = w.o;
+    int rc;
+    if ((rc = blk_reserve(S.din, p.LD.in_total, false)) || (rc = blk_reserve(S.dout, p.LD.out_total, false)) ||
+        (rc = blk_reserve(S.cin, p.LC.in_total, false)) || (rc = blk_reserve(S.cout, p.LC.out_total, false)) ||
+        (rc = blk_reserve(S.chout, 256 + (p.due ? (size_t)p.due->cap * 4 : 0), true))) return rc;
+    if (p.due && (rc = tail_reserve(e, S.ctail))) return rc;
+    if (p.has_reqs && ((rc = blk_reserve(S.creq, p.LR.ent + p.pool * 8, false)) || (rc = blk_reserve(S.creqw, p.w_tmp + p.scan_tmp, false)))) return rc;
+    rafting_inbox_t& d = p.din = stage_inbox(p.LD, S.din.p);
+    if (!p.list) d.gids = nullptr;
+    if (!p.has_sweep) d.row_now = nullptr;
+    if (!p.in->op_c && !p.has_reqs) { d.op_meta = nullptr; d.op_nr = nullptr; }
+    if (!p.in->op_unavail && !p.has_reqs) d.op_ab = nullptr;                // nobody is unavailable
+    if (!p.has_reqs) { d.op_cd = nullptr; d.op_e = nullptr; }
+    d.ent_terms = p.has_reqs ? (const int64_t*)(S.creq.p + p.LR.ent) : nullptr;
+    if (!p.in->ev_c && !p.in->n_esc) { d.ev_meta = nullptr; d.ev_tn = nullptr; d.ev_el = nullptr; }
+    d.rows = (uint32_t)rows; d.n_active = p.list ? (uint32_t)n : 0; d.ent_count = (uint32_t)p.pool;
+    d.flags = (p.has_reqs ? 0u : RAFTING_INBOX_NO_REQUESTS) | (p.list ? RAFTING_INBOX_COMPACT_GROUPS : 0u);
+    p.dout = stage_outbox(p.LD, S.dout.p, nullptr, d.op_meta || d.row_now);
     // the sweep column travels in the copy of the list (whole shard: alone), staged in the slot's pinned block so that the copy
     // is asynchronous whatever memory the caller's column lives in
-    const size_t sweep_at = list ? LD.in_off[1] - LD.in_off[0] : 0;
-    if (has_sweep && (rc = blk_reserve(S.chin, sweep_at + rows * 8, true))) return rc;
-    if (has_reqs && ((rc = blk_reserve(S.creq, LR.ent + pool * 8, false)) || (rc = blk_reserve(S.creqw, w_tmp + scan_tmp, false)))) return rc;
-    // ---- H2D: the wire columns as they are ----
-    CInD ci; ci.rows = (uint32_t)rows; ci.n_esc = in->n_esc;
-    ci.row_base = (const int64_t*)(S.cin.p + LC.row_base); ci.op_c = nullptr; ci.op_unavail = nullptr; ci.ev_c = nullptr;
-    ci.esc = (const rafting_cesc_in_t*)(S.cin.p + LC.esc);
-    {
-        const uint8_t* hb = (const uint8_t*)in->row_base - LC.row_base;      // where the block would start on the host
-        const bool one_block = (!in->op_c || (const uint8_t*)in->op_c == hb + LC.op_c) && (!in->op_unavail || (const uint8_t*)in->op_unavail == hb + LC.op_un) &&
-                               (!in->ev_c || (const uint8_t*)in->ev_c == hb + LC.ev_c) && (!in->n_esc || (const uint8_t*)in->esc == hb + LC.esc) &&
-                               in->op_c && in->ev_c;
-        if (one_block) {
-            const size_t span = in->n_esc ? LC.esc + (size_t)in->n_esc * sizeof(rafting_cesc_in_t)
-                                : (in->op_unavail ? LC.op_un + rows * n * 2 : LC.ev_c + rows * n * F * 4);
-            CU(cudaMemcpyAsync(S.cin.p, hb, span, cudaMemcpyHostToDevice, H->s_h2d));
-            ci.op_c = (const uint32_t*)(S.cin.p + LC.op_c); ci.ev_c = (const uint32_t*)(S.cin.p + LC.ev_c);
-            if (in->op_unavail) ci.op_unavail = (const uint16_t*)(S.cin.p + LC.op_un);
-        } else {
-            CU(cudaMemcpyAsync(S.cin.p + LC.row_base, in->row_base, rows * 8, cudaMemcpyHostToDevice, H->s_h2d));
-            if (in->op_c) { CU(cudaMemcpyAsync(S.cin.p + LC.op_c, in->op_c, rows * n * 4, cudaMemcpyHostToDevice, H->s_h2d)); ci.op_c = (const uint32_t*)(S.cin.p + LC.op_c); }
-            if (in->op_c && in->op_unavail) { CU(cudaMemcpyAsync(S.cin.p + LC.op_un, in->op_unavail, rows * n * 2, cudaMemcpyHostToDevice, H->s_h2d)); ci.op_unavail = (const uint16_t*)(S.cin.p + LC.op_un); }
-            if (in->ev_c) { CU(cudaMemcpyAsync(S.cin.p + LC.ev_c, in->ev_c, rows * n * F * 4, cudaMemcpyHostToDevice, H->s_h2d)); ci.ev_c = (const uint32_t*)(S.cin.p + LC.ev_c); }
-            if (in->n_esc) CU(cudaMemcpyAsync(S.cin.p + LC.esc, in->esc, (size_t)in->n_esc * sizeof(rafting_cesc_in_t), cudaMemcpyHostToDevice, H->s_h2d));
-        }
+    p.sweep_at = p.list && p.has_sweep ? (size_t)((const uint8_t*)d.row_now - (const uint8_t*)d.gids) : 0;
+    if (p.has_sweep && (rc = blk_reserve(S.chin, p.sweep_at + rows * 8, true))) return rc;
+    return RAFTING_OK;
+}
+
+// H2D on the slot's copy stream: the wire columns as they are, the request list, the active list and the sweep column
+static int compact_upload(rafting_engine_t* e, Slot& S, const CompactStep& p) {
+    HostPath* H = hp(e);
+    const rafting_cinbox_t* in = p.in; const rafting_creqs_t* q = p.reqs; const CLayout& LC = p.LC;
+    const size_t rows = p.rows, n = p.n;
+    const WireCol cols[] = {{in->row_base, LC.row_base, rows * 8}, {in->op_c, LC.op_c, rows * n * 4}, {in->ev_c, LC.ev_c, rows * n * e->F * 4},
+                            {in->op_unavail, LC.op_un, rows * n * 2}, {in->esc, LC.esc, (size_t)in->n_esc * sizeof(rafting_cesc_in_t)}};
+    // only an inbox with both op_c and ev_c counts as a block: its one copy spans every column before the last present one
+    if (int rc = wire_copy(cols, 5, in->op_c && in->ev_c ? wire_block(cols, 5) : nullptr, S.cin.p, cudaMemcpyHostToDevice, H->s_h2d)) return rc;
+    if (p.has_reqs) {                                                          // the request list: one copy when carved as laid out
+        const WireCol rcols[] = {{q->req, p.LR.req, p.n_req * sizeof(rafting_creq_t)}, {q->op_esc, p.LR.esc, p.n_oesc * sizeof(rafting_cesc_op_t)},
+                                 {q->ent_terms, p.LR.ent, p.ent_esc * 8}};
+        if (int rc = wire_copy(rcols, 3, wire_block(rcols, 3), S.creq.p, cudaMemcpyHostToDevice, H->s_h2d)) return rc;
     }
-    if (has_reqs) {                                                            // the request list: one copy when carved as laid out
-        const uint8_t* hb = n_req ? (const uint8_t*)reqs->req - LR.req : (const uint8_t*)reqs->op_esc - LR.esc;
-        const bool one_block = (!n_req || (const uint8_t*)reqs->req == hb + LR.req) && (!n_oesc || (const uint8_t*)reqs->op_esc == hb + LR.esc) &&
-                               (!ent_esc || (const uint8_t*)reqs->ent_terms == hb + LR.ent);
-        if (one_block) CU(cudaMemcpyAsync(S.creq.p, hb, LR.total, cudaMemcpyHostToDevice, H->s_h2d));
-        else {
-            if (n_req) CU(cudaMemcpyAsync(S.creq.p + LR.req, reqs->req, n_req * sizeof(rafting_creq_t), cudaMemcpyHostToDevice, H->s_h2d));
-            if (n_oesc) CU(cudaMemcpyAsync(S.creq.p + LR.esc, reqs->op_esc, n_oesc * sizeof(rafting_cesc_op_t), cudaMemcpyHostToDevice, H->s_h2d));
-            if (ent_esc) CU(cudaMemcpyAsync(S.creq.p + LR.ent, reqs->ent_terms, ent_esc * 8, cudaMemcpyHostToDevice, H->s_h2d));
-        }
-    }
-    ActiveD act; act.gids = nullptr; act.n = (uint32_t)n;
-    if (list) act.gids = (const uint32_t*)(S.din.p + LD.in_off[0]);
-    if (has_sweep) {                                                           // [gids | pad] sweep: one copy
-        if (list && n_listed) memcpy(S.chin.p, gids, n_listed * 4);
-        memcpy(S.chin.p + sweep_at, sweep, rows * 8);
-        CU(cudaMemcpyAsync(S.din.p + LD.in_off[1] - sweep_at, S.chin.p, sweep_at + rows * 8, cudaMemcpyHostToDevice, H->s_h2d));
-    } else if (list) {
-        CU(cudaMemcpyAsync((void*)act.gids, gids, n * 4, cudaMemcpyHostToDevice, H->s_h2d));
+    if (p.has_sweep) {                                                         // [gids | pad] sweep: one copy
+        if (p.list && p.n_listed) memcpy(S.chin.p, p.gids, p.n_listed * 4);
+        memcpy(S.chin.p + p.sweep_at, p.sweep, rows * 8);
+        CU(cudaMemcpyAsync((uint8_t*)p.din.row_now - p.sweep_at, S.chin.p, p.sweep_at + rows * 8, cudaMemcpyHostToDevice, H->s_h2d));
+    } else if (p.list) {
+        CU(cudaMemcpyAsync((void*)p.din.gids, p.gids, n * 4, cudaMemcpyHostToDevice, H->s_h2d));
     }
     CU(cudaEventRecord(S.ev_h2d, H->s_h2d));
-    // ---- unpack -> step -> pack on the engine's stream ----
-    InboxD di; memset(&di, 0, sizeof(di));
-    di.rows = (uint32_t)rows; di.n = (uint32_t)n; di.flags = has_reqs ? 0u : RAFTING_INBOX_NO_REQUESTS;
-    if (list) { di.gids = act.gids; di.flags |= RAFTING_INBOX_COMPACT_GROUPS; }
-    if (has_sweep) di.row_now = (const int64_t*)(S.din.p + LD.in_off[1]);
-    if (in->op_c || has_reqs) {
-        di.op_meta = (const uint64_t*)(S.din.p + LD.in_off[2]); di.op_nr = (const i64x2*)(S.din.p + LD.in_off[3]);
-        if (in->op_unavail || has_reqs) di.op_ab = (const i64x2*)(S.din.p + LD.in_off[4]);   // else nobody is unavailable
-    }
-    if (has_reqs) {
-        di.op_cd = (const i64x2*)(S.din.p + LD.in_off[5]); di.op_e = (const int64_t*)(S.din.p + LD.in_off[6]);
-        di.ent_terms = (const int64_t*)(S.creq.p + LR.ent); di.ent_count = (uint32_t)pool;
-    }
-    if (in->ev_c || in->n_esc) {
-        di.ev_meta = (const uint64_t*)(S.din.p + LD.in_off[8]); di.ev_tn = (const i64x2*)(S.din.p + LD.in_off[9]); di.ev_el = (const i64x2*)(S.din.p + LD.in_off[10]);
-    }
-    OutboxD dov; memset(&dov, 0, sizeof(dov));
-    dov.rep_meta = (uint32_t*)(S.dout.p + LD.out_off[0]); dov.rep_term = (int64_t*)(S.dout.p + LD.out_off[1]);
-    dov.plan_meta = (uint64_t*)(S.dout.p + LD.out_off[2]); dov.plan_pp = (i64x2*)(S.dout.p + LD.out_off[3]);
-    dov.plan_lc = (i64x2*)(S.dout.p + LD.out_off[4]); dov.plan_epoch = (int64_t*)(S.dout.p + LD.out_off[5]);
-    dov.ballot_meta = (uint64_t*)(S.dout.p + LD.out_off[6]); dov.ballot_term = (int64_t*)(S.dout.p + LD.out_off[7]);
-    dov.ballot_last = (i64x2*)(S.dout.p + LD.out_off[8]); dov.commit_index = (int64_t*)(S.dout.p + LD.out_off[9]);
-    dov.current_term = (int64_t*)(S.dout.p + LD.out_off[10]); dov.role_word = (uint32_t*)(S.dout.p + LD.out_off[11]);
-    dov.incarnation = (uint32_t*)(S.dout.p + LD.out_off[12]); dov.err_word = (uint32_t*)(S.dout.p + LD.out_off[13]);
-    dov.last_entry = (i64x2*)(S.dout.p + LD.out_off[14]);
-    dov.flags = (uint32_t*)(S.dout.p + LD.flags_off);
-    if (!in->op_c && !has_reqs && !has_sweep) { dov.rep_meta = nullptr; dov.rep_term = nullptr; dov.plan_meta = nullptr; dov.plan_pp = nullptr; dov.plan_lc = nullptr; dov.plan_epoch = nullptr; }
+    return RAFTING_OK;
+}
+
+// unpack -> step -> pack on the engine's stream, behind the slot's H2D copies
+static int compact_run(rafting_engine_t* e, Slot& S, const CompactStep& p) {
+    using namespace rafting;
+    const rafting_cinbox_t* in = p.in; const CLayout& LC = p.LC;
+    const size_t rows = p.rows, NF = p.n * e->F;
+    CInD ci; ci.rows = (uint32_t)rows; ci.n_esc = in->n_esc;
+    ci.row_base = (const int64_t*)(S.cin.p + LC.row_base); ci.esc = (const rafting_cesc_in_t*)(S.cin.p + LC.esc);
+    ci.op_c = in->op_c ? (const uint32_t*)(S.cin.p + LC.op_c) : nullptr;
+    ci.op_unavail = in->op_unavail ? (const uint16_t*)(S.cin.p + LC.op_un) : nullptr;
+    ci.ev_c = in->ev_c ? (const uint32_t*)(S.cin.p + LC.ev_c) : nullptr;
+    InboxD di; OutboxD dov;
+    to_dev_views(&p.din, &p.dout, e->G, (uint32_t*)(S.dout.p + p.LD.flags_off), di, dov);
+    ActiveD act; act.gids = di.gids; act.n = (uint32_t)p.n;
     COutD co;
     co.plan_c = (uint32_t*)(S.cout.p + LC.plan_c); co.rep_c = (uint8_t*)(S.cout.p + LC.rep_c);
     co.commit_index = (int64_t*)(S.cout.p + LC.commit); co.current_term = (int64_t*)(S.cout.p + LC.term); co.role_word = (uint32_t*)(S.cout.p + LC.role);
     co.incarnation = (uint32_t*)(S.cout.p + LC.inc); co.err_word = (uint32_t*)(S.cout.p + LC.err); co.last_entry = (i64x2*)(S.cout.p + LC.last);
     co.epoch = (i64x2*)(S.cout.p + LC.epoch); co.counts = (uint32_t*)(S.cout.p + LC.counts);
-    co.esc = (rafting_cesc_out_t*)(S.cout.p + LC.esc_out); co.esc_cap = out->esc_cap; co.compact_replies = reqs != nullptr;
-    const uint32_t NF = (uint32_t)(n * F), blocks = (NF + 255u) / 256u;
+    co.esc = (rafting_cesc_out_t*)(S.cout.p + LC.esc_out); co.esc_cap = p.out->esc_cap; co.compact_replies = p.reqs != nullptr;
+    const uint32_t blocks = (uint32_t)((NF + 255u) / 256u);
     CU(cudaStreamWaitEvent(e->stream, S.ev_h2d, 0));
     CU(cudaMemsetAsync(dov.flags, 0, 16, e->stream));
     CU(cudaMemsetAsync(co.counts, 0, 16, e->stream));
-    if (due) {                                                                 // the tail of the list, and counts[3]
+    if (p.due) {                                                               // the tail of the list, and counts[3]
         int64_t until = 0;
-        for (size_t r = 0; r < rows; r++) until = sweep[r] > until ? sweep[r] : until;
-        if ((rc = tail_select(e, S.ctail.p, until, (uint32_t*)act.gids, due->n_host, due->cap, co.counts + 3))) {
-            cudaStreamSynchronize(H->s_h2d); return rc;
-        }
+        for (size_t r = 0; r < rows; r++) until = p.sweep[r] > until ? p.sweep[r] : until;
+        if (int rc = tail_select(e, S.ctail.p, until, (uint32_t*)act.gids, p.due->n_host, p.due->cap, co.counts + 3)) return rc;
     }
     InboxW dw;                                                                // unpack writes what the step kernel reads
     dw.op_meta = (uint64_t*)di.op_meta; dw.op_nr = (i64x2*)di.op_nr; dw.op_ab = (i64x2*)di.op_ab;
     dw.ev_meta = (uint64_t*)di.ev_meta; dw.ev_tn = (i64x2*)di.ev_tn; dw.ev_el = (i64x2*)di.ev_el;
     dw.op_cd = (i64x2*)di.op_cd; dw.op_e = (int64_t*)di.op_e; dw.ent_terms = (int64_t*)di.ent_terms;
-    auto* unpack = list ? (el ? unpack_kernel<true, true> : unpack_kernel<false, true>) : (el ? unpack_kernel<true, false> : unpack_kernel<false, false>);
-    unpack<<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits, act);
-    if (in->ev_c == nullptr && in->n_esc) CU(cudaMemsetAsync((void*)di.ev_meta, 0, rows * n * F * 8, e->stream));
-    if (in->n_esc) unpack_escapes_kernel<<<(in->n_esc + 255u) / 256u, 256, 0, e->stream>>>(ci, dw, (uint32_t)(rows * n * F));
-    if (has_reqs) {
+    UNPACK[p.el][p.list]<<<blocks, 256, 0, e->stream>>>(e->T, ci, dw, e->compact->table, e->compact->tinc, e->compact->bits, act);
+    if (in->ev_c == nullptr && in->n_esc) CU(cudaMemsetAsync((void*)di.ev_meta, 0, rows * NF * 8, e->stream));
+    if (in->n_esc) unpack_escapes_kernel<<<(in->n_esc + 255u) / 256u, 256, 0, e->stream>>>(ci, dw, (uint32_t)(rows * NF));
+    if (p.has_reqs) {
         CReqD q;
-        q.n_req = (uint32_t)n_req; q.n_esc = (uint32_t)n_oesc; q.slots = (uint32_t)(rows * n);
-        q.req = (const rafting_creq_t*)(S.creq.p + LR.req); q.esc = (const rafting_cesc_op_t*)(S.creq.p + LR.esc);
+        q.n_req = (uint32_t)p.n_req; q.n_esc = (uint32_t)p.n_oesc; q.slots = (uint32_t)(rows * p.n);
+        q.req = (const rafting_creq_t*)(S.creq.p + p.LR.req); q.esc = (const rafting_cesc_op_t*)(S.creq.p + p.LR.esc);
         q.row_base = ci.row_base; q.op_c = ci.op_c;
-        q.ent_count = (uint32_t)ent_esc; q.pool_end = (uint32_t)pool;
-        q.order = (uint32_t*)S.creqw.p; q.counts = (uint64_t*)(S.creqw.p + w_counts); q.offs = (uint64_t*)(S.creqw.p + w_offs);
-        const uint32_t most = (uint32_t)(n_req > n_oesc ? n_req : n_oesc);
+        q.ent_count = (uint32_t)p.ent_esc; q.pool_end = (uint32_t)p.pool;
+        q.order = (uint32_t*)S.creqw.p; q.counts = (uint64_t*)(S.creqw.p + p.w_counts); q.offs = (uint64_t*)(S.creqw.p + p.w_offs);
+        const uint32_t most = (uint32_t)(p.n_req > p.n_oesc ? p.n_req : p.n_oesc);
         CU(cudaMemsetAsync(q.order, 0, 4, e->stream));
         creq_prepare_kernel<<<(most + 255u) / 256u, 256, 0, e->stream>>>(q);
-        if (n_req) { size_t tb = scan_tmp; CU(cub::DeviceScan::ExclusiveSum(S.creqw.p + w_tmp, tb, q.counts, q.offs, (int)n_req, e->stream)); }
-        const uint32_t rq_blocks = (uint32_t)((n_req + n_oesc + 255u) / 256u);
-        if (el) unpack_requests_kernel<true><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)n);
-        else unpack_requests_kernel<false><<<rq_blocks, 256, 0, e->stream>>>(q, dw, (uint32_t)n);
+        if (p.n_req) { size_t tb = p.scan_tmp; CU(cub::DeviceScan::ExclusiveSum(S.creqw.p + p.w_tmp, tb, q.counts, q.offs, (int)p.n_req, e->stream)); }
+        UNPACK_REQUESTS[p.el]<<<(uint32_t)((p.n_req + p.n_oesc + 255u) / 256u), 256, 0, e->stream>>>(q, dw, (uint32_t)p.n);
     }
     CU(cudaGetLastError());
-    rc = launch_step(e, di, dov, e->stream);
-    if (rc) { cudaStreamSynchronize(H->s_h2d); return rc; }
-    auto* pack = list ? (el ? (pt ? pack_kernel<true, true, true> : pack_kernel<true, false, true>) : (pt ? pack_kernel<false, true, true> : pack_kernel<false, false, true>))
-                      : (el ? (pt ? pack_kernel<true, true, false> : pack_kernel<true, false, false>) : (pt ? pack_kernel<false, true, false> : pack_kernel<false, false, false>));
-    pack<<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits, act);
+    if (int rc = launch_step(e, di, dov, e->stream)) return rc;
+    PACK[p.el][p.pt][p.list]<<<blocks, 256, 0, e->stream>>>(e->T, (uint32_t)rows, dov, co, e->compact->table, e->compact->tinc, e->compact->bits, act);
     CU(cudaGetLastError());
     CU(cudaEventRecord(S.ev_kernel, e->stream));
+    return RAFTING_OK;
+}
+
+// One compact step in `slot`: over the whole shard (gids == nullptr, n = G), or over the n groups gids[0 .. n) that the caller
+// has checked (strictly increasing, each < G).  Every wire column and every dense staging column holds n groups per row.
+// sweep (host, [rows], may be null): the step's row_now column (rafting_step_begin_compact_sweep).
+// due (rafting_step_begin_compact_due): gids holds due->n_host entries and n_active = n_host + cap; the device writes the
+// rest of the list before unpack_kernel reads it.
+static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
+                         const rafting_coutbox_t* out, uint32_t flags, uint32_t n_active, const uint32_t* gids,
+                         const int64_t* sweep = nullptr, const DueTail* due = nullptr) {
+    CompactStep p = {in, reqs, out, gids, sweep, due};
+    int rc = compact_check(e, slot, flags, n_active, p);
+    if (rc || (rc = compact_reserve(e, hp(e)->slot[slot], p))) return rc;   // refused: nothing is enqueued, the slot stays free
+    HostPath* H = hp(e); Slot& S = H->slot[slot];
+    if ((rc = compact_upload(e, S, p)) || (rc = compact_run(e, S, p))) { cudaStreamSynchronize(H->s_h2d); return rc; }
     // ---- D2H: every wire column + the counters; the escape list only when the counters say it holds something ----
+    // the first escape records always travel with the columns (a steady-state launch produces a handful): fetching them
+    // on demand at wait time would have to drain the D2H stream, i.e. wait for the copies of every LATER launch as well
     CU(cudaStreamWaitEvent(H->s_d2h, S.ev_kernel, 0));
-    const uint32_t esc_inline = out->esc_cap < CESC_INLINE ? out->esc_cap : CESC_INLINE;
-    uint32_t* counts_land = (uint32_t*)S.chout.p;
-    {
-        uint8_t* hb = (uint8_t*)out->plan_c - LC.plan_c;
-        const bool one_block = (uint8_t*)out->rep_c == hb + LC.rep_c && (uint8_t*)out->commit_index == hb + LC.commit && (uint8_t*)out->current_term == hb + LC.term &&
-                               (uint8_t*)out->role_word == hb + LC.role && (uint8_t*)out->incarnation == hb + LC.inc && (uint8_t*)out->err_word == hb + LC.err &&
-                               (uint8_t*)out->last_entry == hb + LC.last && (uint8_t*)out->epoch == hb + LC.epoch && (uint8_t*)out->counts == hb + LC.counts &&
-                               (!out->esc_cap || (uint8_t*)out->esc == hb + LC.esc_out);
-        if (one_block) {
-            // columns, counters and the first escape records: one copy (the counters land in the caller's block directly)
-            CU(cudaMemcpyAsync(hb, S.cout.p, LC.esc_out + (size_t)esc_inline * sizeof(rafting_cesc_out_t), cudaMemcpyDeviceToHost, H->s_d2h));
-            counts_land = out->counts;
-        } else {
-            CU(cudaMemcpyAsync(out->plan_c, co.plan_c, rows * n * F * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->rep_c, co.rep_c, rows * n, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->commit_index, co.commit_index, n * 8, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->current_term, co.current_term, n * 8, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->role_word, co.role_word, n * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->incarnation, co.incarnation, n * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->err_word, co.err_word, n * 4, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->last_entry, co.last_entry, n * 16, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(out->epoch, co.epoch, n * 16, cudaMemcpyDeviceToHost, H->s_d2h));
-            CU(cudaMemcpyAsync(S.chout.p, co.counts, 16, cudaMemcpyDeviceToHost, H->s_d2h));
-            // the first escape records always travel with the columns (a steady-state launch produces a handful): fetching them
-            // on demand at wait time would have to drain the D2H stream, i.e. wait for the copies of every LATER launch as well
-            if (esc_inline) CU(cudaMemcpyAsync(out->esc, co.esc, (size_t)esc_inline * sizeof(rafting_cesc_out_t), cudaMemcpyDeviceToHost, H->s_d2h));
-        }
-    }
-    if (due) CU(cudaMemcpyAsync(S.chout.p + 256, act.gids + due->n_host, (size_t)due->cap * 4, cudaMemcpyDeviceToHost, H->s_d2h));
+    const CLayout& LC = p.LC; const size_t rows = p.rows, n = p.n;
+    const uint32_t esc_inline = out->esc_cap < rafting::CESC_INLINE ? out->esc_cap : rafting::CESC_INLINE;
+    WireCol cols[] = {{out->plan_c, LC.plan_c, rows * n * e->F * 4}, {out->rep_c, LC.rep_c, rows * n}, {out->commit_index, LC.commit, n * 8},
+                      {out->current_term, LC.term, n * 8}, {out->role_word, LC.role, n * 4}, {out->incarnation, LC.inc, n * 4},
+                      {out->err_word, LC.err, n * 4}, {out->last_entry, LC.last, n * 16}, {out->epoch, LC.epoch, n * 16},
+                      {out->counts, LC.counts, 16}, {out->esc, LC.esc_out, (size_t)esc_inline * sizeof(rafting_cesc_out_t)}};
+    WireCol& counts = cols[9];
+    uint8_t* hb = wire_block(cols, 11);
+    if (!hb) counts.h = S.chout.p;                                            // column by column: into the slot's pinned block
+    if ((rc = wire_copy(cols, 11, hb, S.cout.p, cudaMemcpyDeviceToHost, H->s_d2h))) return rc;
+    if (due) CU(cudaMemcpyAsync(S.chout.p + 256, p.din.gids + due->n_host, (size_t)due->cap * 4, cudaMemcpyDeviceToHost, H->s_d2h));
     CU(cudaEventRecord(S.ev_done, H->s_d2h));
-    S.compact_step = true; S.c_host = *out; S.c_counts_pinned = counts_land; S.c_esc_dev = co.esc;
+    S.compact_step = true; S.c_host = *out; S.c_counts_pinned = (uint32_t*)counts.h; S.c_esc_dev = S.cout.p + LC.esc_out;
     S.c_tail_user = due ? due->tail_out : nullptr; S.c_tail_n = due ? due->cap : 0;
-    S.dev_out = rafting_outbox_t(); memset(&S.dev_out, 0, sizeof(S.dev_out));
-    S.dev_out.rep_meta = dov.rep_meta; S.dev_out.rep_term = dov.rep_term; S.dev_out.plan_meta = dov.plan_meta;
-    S.dev_out.plan_pp = (rafting_i64x2_t*)dov.plan_pp; S.dev_out.plan_lc = (rafting_i64x2_t*)dov.plan_lc; S.dev_out.plan_epoch = dov.plan_epoch;
-    S.dev_out.ballot_meta = dov.ballot_meta; S.dev_out.ballot_term = dov.ballot_term; S.dev_out.ballot_last = (rafting_i64x2_t*)dov.ballot_last;
-    S.dev_out.commit_index = dov.commit_index; S.dev_out.current_term = dov.current_term; S.dev_out.role_word = dov.role_word;
-    S.dev_out.incarnation = dov.incarnation; S.dev_out.err_word = dov.err_word; S.dev_out.last_entry = (rafting_i64x2_t*)dov.last_entry;
-    S.rows_ = rows; S.n_ = n; S.gcols_ = n;
+    S.dev_out = p.dout; S.rows_ = rows; S.n_ = n;
     S.inflight = true;
     return RAFTING_OK;
 }
@@ -675,18 +698,6 @@ extern "C" int rafting_step_begin_compact_ex(rafting_engine_t* e, uint32_t slot,
     return compact_begin(e, slot, in, reqs, out, flags, 0, nullptr);
 }
 
-// The list is checked in full before anything is enqueued: a lane's tag bitmap must have exactly one owning thread, and the
-// in-flight table is indexed by gid, so a duplicate or an id past max_groups would race on it or index past it.
-static int check_active_list(rafting_engine_t* e, uint32_t n_active, const uint32_t* gids) {
-    if (!e || !gids) return fail(RAFTING_E_INVAL, "bad argument");
-    if (n_active == 0) return fail(RAFTING_E_INVAL, "an active list holds at least one group");
-    if (n_active > e->G) return fail(RAFTING_E_CAPACITY, "n_active %u > max_groups %u", n_active, e->G);
-    for (uint32_t k = 0; k < n_active; k++) {
-        if (gids[k] >= e->G) return fail(RAFTING_E_INVAL, "gids[%u] = %u is not below max_groups", k, gids[k]);
-        if (k > 0 && gids[k] <= gids[k - 1]) return fail(RAFTING_E_INVAL, "gids must be strictly increasing (gids[%u] = %u)", k, gids[k]);
-    }
-    return RAFTING_OK;
-}
 extern "C" int rafting_step_begin_compact_active(rafting_engine_t* e, uint32_t slot, uint32_t n_active, const uint32_t* gids,
                                                  const rafting_cinbox_t* in, const rafting_creqs_t* reqs, const rafting_coutbox_t* out,
                                                  uint32_t flags) {
@@ -699,7 +710,6 @@ extern "C" int rafting_step_begin_compact_sweep(rafting_engine_t* e, uint32_t sl
                                                 const rafting_cinbox_t* in, const rafting_creqs_t* reqs, const rafting_coutbox_t* out,
                                                 uint32_t flags) {
     if (gids) { if (int rc = check_active_list(e, n_active, gids)) return rc; }
-    else n_active = 0;
     return compact_begin(e, slot, in, reqs, out, flags, n_active, gids, sweep);
 }
 
@@ -708,14 +718,6 @@ extern "C" int rafting_step_begin_compact_sweep(rafting_engine_t* e, uint32_t sl
 extern "C" int rafting_step_begin_compact_due(rafting_engine_t* e, uint32_t slot, uint32_t n_host, const uint32_t* gids, uint32_t cap,
                                               const int64_t* sweep, const rafting_cinbox_t* in, const rafting_creqs_t* reqs,
                                               const rafting_coutbox_t* out, uint32_t* tail_out, uint32_t flags) {
-    if (!e || !in || !sweep || !tail_out || (n_host && !gids)) return fail(RAFTING_E_INVAL, "bad argument");
-    if (cap == 0) return fail(RAFTING_E_INVAL, "a due step's tail holds at least one group (cap >= 1)");
-    if ((uint64_t)n_host + cap > e->G)
-        return fail(RAFTING_E_CAPACITY, "n_host %u + cap %u > max_groups %u: not enough groups outside the list to fill the tail", n_host, cap, e->G);
-    if (n_host) { if (int rc = check_active_list(e, n_host, gids)) return rc; }
-    bool has_sweep = false;
-    for (uint32_t r = 0; r < in->rows && r < e->cfg.max_rows; r++) has_sweep |= sweep[r] != 0;
-    if (!has_sweep) return fail(RAFTING_E_INVAL, "a due step needs a sweep row");
     const DueTail due = {n_host, cap, tail_out};
     return compact_begin(e, slot, in, reqs, out, flags, n_host + cap, gids, sweep, &due);
 }
@@ -748,7 +750,7 @@ extern "C" int rafting_step_fetch_dense(rafting_engine_t* e, uint32_t slot, cons
         const ColDesc& c = OUT_COLS[k];
         void* h = out_ptr(out, c); void* d = out_ptr(&S.dev_out, c);
         if (!h || !d) continue;
-        CU(cudaMemcpyAsync(h, d, col_bytes(c, S.rows_, S.n_, e->F, S.gcols_, 0, 0), cudaMemcpyDeviceToHost, H->s_d2h));
+        CU(cudaMemcpyAsync(h, d, col_bytes(c, S.rows_, S.n_, e->F, S.n_, 0, 0), cudaMemcpyDeviceToHost, H->s_d2h));
     }
     CU(cudaStreamSynchronize(H->s_d2h));
     return RAFTING_OK;

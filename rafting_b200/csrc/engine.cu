@@ -358,7 +358,7 @@ static int launch_step(rafting_engine* e, const InboxD& in0, const OutboxD& out,
     return RAFTING_OK;
 }
 
-static void to_dev_views(const rafting_inbox_t* in, const rafting_outbox_t* out, uint32_t G, InboxD& di, OutboxD& dout) {
+static void to_dev_views(const rafting_inbox_t* in, const rafting_outbox_t* out, uint32_t G, uint32_t* flags, InboxD& di, OutboxD& dout) {
     di.rows = in->rows; di.n = in->gids ? in->n_active : G; di.gids = in->gids; di.row_now = in->row_now;
     di.op_meta = in->op_meta; di.op_nr = (const i64x2*)in->op_nr; di.op_ab = (const i64x2*)in->op_ab;
     di.op_cd = (const i64x2*)in->op_cd; di.op_e = in->op_e; di.ent_terms = in->ent_terms; di.ent_count = in->ent_count; di.flags = in->flags;
@@ -367,7 +367,7 @@ static void to_dev_views(const rafting_inbox_t* in, const rafting_outbox_t* out,
     dout.plan_pp = (i64x2*)out->plan_pp; dout.plan_lc = (i64x2*)out->plan_lc; dout.plan_epoch = out->plan_epoch;
     dout.ballot_meta = out->ballot_meta; dout.ballot_term = out->ballot_term; dout.ballot_last = (i64x2*)out->ballot_last;
     dout.commit_index = out->commit_index; dout.current_term = out->current_term; dout.role_word = out->role_word;
-    dout.incarnation = out->incarnation; dout.err_word = out->err_word; dout.last_entry = (i64x2*)out->last_entry; dout.flags = nullptr;
+    dout.incarnation = out->incarnation; dout.err_word = out->err_word; dout.last_entry = (i64x2*)out->last_entry; dout.flags = flags;
 }
 
 extern "C" int rafting_step_device(rafting_engine_t* e, const rafting_inbox_t* in, const rafting_outbox_t* out, void* stream) {
@@ -375,7 +375,7 @@ extern "C" int rafting_step_device(rafting_engine_t* e, const rafting_inbox_t* i
     if (in->gids && in->n_active > e->G) return fail(RAFTING_E_CAPACITY, "n_active > max_groups");
     CU(cudaSetDevice(e->cfg.device));
     InboxD di; OutboxD dout;
-    to_dev_views(in, out, e->G, di, dout);
+    to_dev_views(in, out, e->G, nullptr, di, dout);
     return launch_step(e, di, dout, stream ? (cudaStream_t)stream : e->stream);
 }
 
@@ -438,28 +438,49 @@ template <typename S> static void*& out_ptr(S* st, const ColDesc& c) { return *(
 // so adjacent columns travel in a single cudaMemcpyAsync (a leased leader step is 1 copy up, 1 copy down).
 static const int IN_ORDER[N_IN]   = {2, 3, 8, 9, 10, 4, 5, 6, 7, 0, 1};     // op_meta op_nr ev_meta ev_tn ev_el op_ab op_cd op_e ent gids row_now
 static const int OUT_ORDER[N_OUT] = {0, 2, 3, 4, 5, 6, 9, 10, 11, 12, 13, 14, 1, 7, 8};   // ... dense ..., then rep_term ballot_term ballot_last
+// carves one block into 256-byte aligned parts: take(bytes) returns the next part's offset, o is where the block ends so far
+struct Carve { size_t o = 0; size_t take(size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; } };
 struct Layout { size_t in_off[N_IN], out_off[N_OUT], flags_off, in_total, out_total; };
 // gcols = entries of a per-group outbox column: max_groups, or n under RAFTING_INBOX_COMPACT_GROUPS
 static Layout make_layout(size_t rows, size_t n, size_t F, size_t gcols, size_t nact, size_t ent) {
     const size_t G = gcols;
-    Layout L; size_t off = 0;
-    for (int q = 0; q < N_IN; q++) { const int k = IN_ORDER[q]; L.in_off[k] = off; off += (col_bytes(IN_COLS[k], rows, n, F, G, nact, ent + 1) + 255) & ~(size_t)255; }
-    L.in_total = off; off = 0;
+    Layout L; Carve in, out;
+    for (int q = 0; q < N_IN; q++) { const int k = IN_ORDER[q]; L.in_off[k] = in.take(col_bytes(IN_COLS[k], rows, n, F, G, nact, ent + 1)); }
+    L.in_total = in.o;
     for (int q = 0; q < N_OUT; q++) {
         const int k = OUT_ORDER[q];
-        if (q == N_OUT - 3) { L.flags_off = off; off += 256; }              // the two flag words sit right after the dense columns
-        L.out_off[k] = off; off += (col_bytes(OUT_COLS[k], rows, n, F, G, 0, 0) + 255) & ~(size_t)255;
+        if (q == N_OUT - 3) L.flags_off = out.take(16);                    // the two flag words sit right after the dense columns
+        L.out_off[k] = out.take(col_bytes(OUT_COLS[k], rows, n, F, G, 0, 0));
     }
-    L.out_total = off;
+    L.out_total = out.o;
     return L;
 }
+// Device staging views of one step in the blocks carved by make_layout.  The inbox view has every column at its offset; the
+// caller nulls the ones its step does not carry.  The outbox view has the columns `want` has (every one when want is null),
+// except that without an op or a sweep row nothing can produce replies or plans, so those columns stay null.
+static rafting_inbox_t stage_inbox(const Layout& L, uint8_t* blk) {
+    rafting_inbox_t v; memset(&v, 0, sizeof(v));
+    for (int k = 0; k < N_IN; k++) in_ptr(&v, IN_COLS[k]) = blk + L.in_off[k];
+    return v;
+}
+static rafting_outbox_t stage_outbox(const Layout& L, uint8_t* blk, const rafting_outbox_t* want, bool ops) {
+    rafting_outbox_t v; memset(&v, 0, sizeof(v));
+    for (int k = 0; k < N_OUT; k++) {
+        const ColDesc& c = OUT_COLS[k];
+        const bool repOrPlan = c.off <= offsetof(rafting_outbox_t, plan_epoch);
+        if ((!want || out_ptr(want, c)) && (ops || !repOrPlan)) out_ptr(&v, c) = blk + L.out_off[k];
+    }
+    return v;
+}
 struct Blk { uint8_t* p = nullptr; size_t cap = 0; };
+static void blk_free(Blk& b, bool pinned) { if (b.p) { if (pinned) cudaFreeHost(b.p); else cudaFree(b.p); b.p = nullptr; b.cap = 0; } }
 static int blk_reserve(Blk& b, size_t bytes, bool pinned) {
     if (bytes <= b.cap) return 0;
-    if (b.p) { if (pinned) cudaFreeHost(b.p); else cudaFree(b.p); b.p = nullptr; b.cap = 0; }
+    blk_free(b, pinned);
     const size_t cap = bytes + bytes / 4 + 4096;
     if (pinned) { CU(cudaHostAlloc((void**)&b.p, cap, cudaHostAllocDefault)); memset(b.p, 0, cap); }
     else { CU(cudaMalloc((void**)&b.p, cap)); CU(cudaMemset(b.p, 0, cap)); }   // column padding and never-written plan fields travel in the one-block D2H copy: defined bytes
+    if (!pinned) CU(cudaStreamSynchronize(0));        // that memset runs on the legacy stream, which the engine's non-blocking streams do not wait for
     b.cap = cap;
     return 0;
 }
@@ -468,8 +489,8 @@ struct Slot {
     Blk din, dout;                            // device staging (both paths)
     Blk cin, cout, chin, chout;               // compact path: device wire blocks + pinned landing block of the small items
     Blk creq, creqw;                          // compact path: request list + entry pool, and its scan scratch
-    bool compact_step = false;                // the step in flight came through rafting_step_begin_compact[_req]
-    rafting_coutbox_t c_host; size_t c_esc_off = 0; uint32_t* c_counts_pinned = nullptr; void* c_esc_dev = nullptr;
+    bool compact_step = false;                // the step in flight came through one of the rafting_step_begin_compact* calls
+    rafting_coutbox_t c_host; uint32_t* c_counts_pinned = nullptr; void* c_esc_dev = nullptr;
     Blk ctail;                                // rafting_step_begin_compact_due: the tail selection's scratch (timers.cuh)
     uint32_t* c_tail_user = nullptr; uint32_t c_tail_n = 0;   // where the wait copies the tail (landed at chout + 256)
     Blk hin, hout;                            // pinned host staging (leases only), same layout as din / dout
@@ -481,7 +502,6 @@ struct Slot {
     uint32_t lease_gen = 0;
     // of the step in flight (for the sparse columns fetched at wait time)
     rafting_outbox_t host_out; rafting_outbox_t dev_out; size_t rows_ = 0, n_ = 0; const uint32_t* flags_host = nullptr;
-    size_t gcols_ = 0;                        // compact steps: entries of a per-group column (max_groups, or n_active)
 };
 struct HostPath {
     Slot slot[RAFTING_HOST_SLOTS];
@@ -517,17 +537,8 @@ static int hostpath_init(rafting_engine* e) {
 static void hostpath_free(rafting_engine* e) {
     HostPath* H = hp(e);
     for (Slot& s : H->slot) {
-        if (s.din.p) cudaFree(s.din.p);
-        if (s.dout.p) cudaFree(s.dout.p);
-        if (s.hin.p) cudaFreeHost(s.hin.p);
-        if (s.hout.p) cudaFreeHost(s.hout.p);
-        if (s.cin.p) cudaFree(s.cin.p);
-        if (s.cout.p) cudaFree(s.cout.p);
-        if (s.chin.p) cudaFreeHost(s.chin.p);
-        if (s.chout.p) cudaFreeHost(s.chout.p);
-        if (s.creq.p) cudaFree(s.creq.p);
-        if (s.creqw.p) cudaFree(s.creqw.p);
-        if (s.ctail.p) cudaFree(s.ctail.p);
+        for (Blk* b : {&s.din, &s.dout, &s.cin, &s.cout, &s.creq, &s.creqw, &s.ctail}) blk_free(*b, false);
+        for (Blk* b : {&s.hin, &s.hout, &s.chin, &s.chout}) blk_free(*b, true);
         if (s.ev_h2d) cudaEventDestroy(s.ev_h2d);
         if (s.ev_kernel) cudaEventDestroy(s.ev_kernel);
         if (s.ev_done) cudaEventDestroy(s.ev_done);
@@ -579,7 +590,7 @@ static int step_enqueue(rafting_engine* e, uint32_t slot, const rafting_inbox_t*
                               : make_layout(rows, n, F, gcols, in->n_active, in->ent_count);
     int rc;
     if ((rc = blk_reserve(S.din, L.in_total, false)) || (rc = blk_reserve(S.dout, L.out_total, false))) return rc;
-    rafting_inbox_t din = *in; rafting_outbox_t dout; memset(&dout, 0, sizeof(dout));
+    rafting_inbox_t din = *in;
     // ---- H2D ----
     std::vector<CopyItem> up;
     for (int q = 0; q < N_IN; q++) {
@@ -599,20 +610,12 @@ static int step_enqueue(rafting_engine* e, uint32_t slot, const rafting_inbox_t*
     if ((rc = issue_copies(up, true, H->s_h2d, S.hin))) return rc;
     CU(cudaEventRecord(S.ev_h2d, H->s_h2d));
     // ---- kernel ----
-    const bool ops = din.op_meta || din.row_now;
-    for (int k = 0; k < N_OUT; k++) {
-        const ColDesc& c = OUT_COLS[k];
-        bool use = out_ptr(out, c) != nullptr;
-        const bool repOrPlan = c.off <= offsetof(rafting_outbox_t, plan_epoch);
-        if (repOrPlan && !ops) use = false;                                  // nothing can produce replies / plans
-        if (use) out_ptr(&dout, c) = S.dout.p + L.out_off[k];
-    }
+    rafting_outbox_t dout = stage_outbox(L, S.dout.p, out, din.op_meta || din.row_now);
     uint32_t* d_flags = (uint32_t*)(S.dout.p + L.flags_off);
     CU(cudaStreamWaitEvent(e->stream, S.ev_h2d, 0));
     CU(cudaMemsetAsync(d_flags, 0, 16, e->stream));
     InboxD di; OutboxD dov;
-    to_dev_views(&din, &dout, e->G, di, dov);
-    dov.flags = d_flags;
+    to_dev_views(&din, &dout, e->G, d_flags, di, dov);
     rc = launch_step(e, di, dov, e->stream);
     if (rc) { cudaStreamSynchronize(H->s_h2d); return rc; }                  // no copy of this step may outlive the failed call
     CU(cudaEventRecord(S.ev_kernel, e->stream));
@@ -690,12 +693,10 @@ extern "C" int rafting_lease_ex(rafting_engine_t* e, uint32_t rows, uint32_t n_a
     const Layout L = make_layout(rows, n, F, compact ? n : G, n_active, ent_count);
     if ((rc = blk_reserve(S.hin, L.in_total, true)) || (rc = blk_reserve(S.hout, L.out_total, true))) return rc;
     memset(out, 0, sizeof(*out));
-    for (int k = 0; k < N_IN; k++) {
-        const ColDesc& c = IN_COLS[k];
-        in_ptr(&out->in, c) = (c.per == PER_ACTIVE && n_active == 0) ? nullptr : (S.hin.p + L.in_off[k]);
-    }
-    memset(S.hin.p + L.in_off[1], 0, (size_t)rows * 8);                     // row_now: no sweep unless the caller sets it
-    for (int k = 0; k < N_OUT; k++) out_ptr(&out->out, OUT_COLS[k]) = S.hout.p + L.out_off[k];
+    out->in = stage_inbox(L, S.hin.p);
+    if (n_active == 0) out->in.gids = nullptr;
+    memset((void*)out->in.row_now, 0, (size_t)rows * 8);                   // row_now: no sweep unless the caller sets it
+    out->out = stage_outbox(L, S.hout.p, nullptr, true);
     out->in.rows = rows; out->in.n_active = n_active; out->in.ent_count = ent_count; out->in.flags = flags;
     S.compact = compact;
     S.leased = true; S.rows = rows; S.n = (uint32_t)n; S.ent = ent_count; S.list = n_active != 0;

@@ -169,18 +169,16 @@ static int tail_layout(uint32_t G, TailLayout& L) {
     L.nblocks = (G + DUE_TPB - 1) / DUE_TPB;
     size_t scan_tmp = 0;
     CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)L.nblocks));
-    size_t o = 0;
-    auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; };
-    L.member = take((size_t)L.nblocks * TAIL_WARPS * 4); L.mask = take((size_t)L.nblocks * TAIL_WARPS * 8);
-    L.agg = take((size_t)L.nblocks * 8); L.off = take((size_t)L.nblocks * 8); L.tmp = take(scan_tmp);
-    L.total = o;
+    Carve c;
+    L.member = c.take((size_t)L.nblocks * TAIL_WARPS * 4); L.mask = c.take((size_t)L.nblocks * TAIL_WARPS * 8);
+    L.agg = c.take((size_t)L.nblocks * 8); L.off = c.take((size_t)L.nblocks * 8); L.tmp = c.take(scan_tmp);
+    L.total = c.o;
     return RAFTING_OK;
 }
-static int tail_scratch_bytes(uint32_t G, size_t* bytes) {
+static int tail_reserve(rafting_engine* e, Blk& scratch) {
     TailLayout L;
-    if (int rc = tail_layout(G, L)) return rc;
-    *bytes = L.total;
-    return RAFTING_OK;
+    if (int rc = tail_layout(e->G, L)) return rc;
+    return blk_reserve(scratch, L.total, false);
 }
 
 // Enqueues the tail selection on the engine's stream: list[0 .. n_host) is the host's part (device copy), the tail goes to
@@ -201,10 +199,10 @@ static int tail_select(rafting_engine* e, uint8_t* scratch, int64_t until, uint3
     return RAFTING_OK;
 }
 
-// One query slot: device scratch, a mapped pinned block for the result (and the list when the caller's buffer is not mapped)
+// One query slot: device scratch, a pinned (so mapped) block for the result (and the list when the caller's buffer is not mapped)
 struct DueSlot {
-    uint8_t* dev = nullptr; size_t dev_cap = 0;            // mask, block pairs, their scan, CUB's scratch
-    uint8_t* host = nullptr; size_t host_cap = 0;          // mapped pinned: DueResult, then the staged list
+    Blk dev;                                               // mask, block pairs, their scan, CUB's scratch
+    Blk host;                                              // DueResult, then the staged list
     cudaEvent_t ev = nullptr;
     bool inflight = false;
     uint32_t* user = nullptr; uint32_t cap = 0;            // the caller's buffer; staged: copy from host + 256 at the wait
@@ -215,8 +213,8 @@ struct DuePath { DueSlot slot[RAFTING_HOST_SLOTS]; };
 static void due_release(rafting_engine* e) {
     if (!e->due) return;
     for (DueSlot& s : e->due->slot) {
-        if (s.dev) cudaFree(s.dev);
-        if (s.host) cudaFreeHost(s.host);
+        blk_free(s.dev, false);
+        blk_free(s.host, true);
         if (s.ev) cudaEventDestroy(s.ev);
     }
     delete e->due; e->due = nullptr;
@@ -233,13 +231,10 @@ extern "C" int rafting_timers_due_begin(rafting_engine_t* e, uint32_t slot, int6
     const uint32_t nblocks = (e->G + DUE_TPB - 1) / DUE_TPB;
     size_t scan_tmp = 0;
     CU(cub::DeviceScan::ExclusiveScan(nullptr, scan_tmp, (DueAgg*)nullptr, (DueAgg*)nullptr, DueAggOp(), DueAgg{0, 0, I64MAX}, (int)nblocks));
-    const size_t o_mask = 0, o_agg = ((size_t)nblocks * (DUE_TPB / 32) * 4 + 255) & ~(size_t)255;
-    const size_t o_off = o_agg + (((size_t)nblocks * sizeof(DueAgg) + 255) & ~(size_t)255);
-    const size_t o_tmp = o_off + (((size_t)nblocks * sizeof(DueAgg) + 255) & ~(size_t)255), dev_bytes = o_tmp + scan_tmp;
-    if (dev_bytes > S.dev_cap) {
-        if (S.dev) { cudaFree(S.dev); S.dev = nullptr; S.dev_cap = 0; }
-        CU(cudaMalloc((void**)&S.dev, dev_bytes)); S.dev_cap = dev_bytes;
-    }
+    Carve c;
+    const size_t o_mask = c.take((size_t)nblocks * (DUE_TPB / 32) * 4), o_agg = c.take((size_t)nblocks * sizeof(DueAgg));
+    const size_t o_off = c.take((size_t)nblocks * sizeof(DueAgg)), o_tmp = c.o;
+    if (int rc = blk_reserve(S.dev, o_tmp + scan_tmp, false)) return rc;
     // the caller's buffer, if the device can write it (mapped pinned memory); else the slot's staging block
     void* dst = nullptr;
     bool staged = false;
@@ -248,18 +243,14 @@ extern "C" int rafting_timers_due_begin(rafting_engine_t* e, uint32_t slot, int6
         if (cudaPointerGetAttributes(&pa, gids_out) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer) dst = pa.devicePointer;
         else { cudaGetLastError(); staged = true; }
     }
-    const size_t host_bytes = 256 + (staged ? (size_t)cap * 4 : 0);
-    if (host_bytes > S.host_cap) {
-        if (S.host) { cudaFreeHost(S.host); S.host = nullptr; S.host_cap = 0; }
-        CU(cudaHostAlloc((void**)&S.host, host_bytes, cudaHostAllocMapped)); S.host_cap = host_bytes;
-    }
+    if (int rc = blk_reserve(S.host, 256 + (staged ? (size_t)cap * 4 : 0), true)) return rc;
     uint8_t* hdev = nullptr;
-    CU(cudaHostGetDevicePointer((void**)&hdev, S.host, 0));
+    CU(cudaHostGetDevicePointer((void**)&hdev, S.host.p, 0));
     if (staged) dst = hdev + 256;
-    uint32_t* mask = (uint32_t*)(S.dev + o_mask); DueAgg* agg = (DueAgg*)(S.dev + o_agg); DueAgg* off = (DueAgg*)(S.dev + o_off);
+    uint32_t* mask = (uint32_t*)(S.dev.p + o_mask); DueAgg* agg = (DueAgg*)(S.dev.p + o_agg); DueAgg* off = (DueAgg*)(S.dev.p + o_off);
     due_scan_kernel<<<nblocks, DUE_TPB, 0, e->stream>>>(e->T, until_ms, mask, agg);
     size_t tb = scan_tmp;
-    CU(cub::DeviceScan::ExclusiveScan(S.dev + o_tmp, tb, agg, off, DueAggOp(), DueAgg{0, 0, I64MAX}, (int)nblocks, e->stream));
+    CU(cub::DeviceScan::ExclusiveScan(S.dev.p + o_tmp, tb, agg, off, DueAggOp(), DueAgg{0, 0, I64MAX}, (int)nblocks, e->stream));
     due_emit_kernel<<<nblocks, DUE_TPB, 0, e->stream>>>(mask, agg, off, nblocks, (uint32_t*)dst, cap, (DueResult*)hdev);
     CU(cudaGetLastError());
     CU(cudaEventRecord(S.ev, e->stream));
@@ -276,8 +267,8 @@ extern "C" int rafting_timers_due_wait(rafting_engine_t* e, uint32_t slot, uint3
     DueSlot& S = e->due->slot[slot];
     CU(cudaEventSynchronize(S.ev));
     S.inflight = false;
-    const DueResult* r = (const DueResult*)S.host;
-    if (S.staged) memcpy(S.user, S.host + 256, (size_t)(r->n_due < S.cap ? r->n_due : S.cap) * 4);
+    const DueResult* r = (const DueResult*)S.host.p;
+    if (S.staged) memcpy(S.user, S.host.p + 256, (size_t)(r->n_due < S.cap ? r->n_due : S.cap) * 4);
     if (n_due) *n_due = r->n_due;
     if (next_deadline_ms) *next_deadline_ms = r->next;
     return RAFTING_OK;
