@@ -381,6 +381,36 @@ int rafting_group_close    (rafting_engine_t* e, uint32_t gid);
  * RAFTING_TERM_RUNS runs (RAFTING_E_CAPACITY beyond: compact the log first). */
 int rafting_group_load_runs(rafting_engine_t* e, uint32_t gid, const rafting_i64x2_t* runs, uint32_t n_runs);
 
+/* Open, restart and close groups in step-stream order, while steps are in flight (ContextManager.buildContext / exitContext
+ * issued by a pipelined pump between two step begins).
+ *   Ordering: the edits are enqueued on the engine's step stream.  Every step, due query and edit begun before the call sees
+ *     the tables without them, everything begun after it sees them.  Host, compact, active, sweep and due steps may be in
+ *     flight: the call never returns RAFTING_E_BUSY for that and never synchronises the step stream.  Steps enqueued on a
+ *     CALLER's stream through rafting_step_device must be ordered by the caller, as for rafting_group_open.
+ *   Effect: at its place in the stream an OPEN leaves the gid exactly as rafting_group_open(init), followed by
+ *     rafting_group_load_runs(runs, n_runs) when n_runs > 0, would after a drain; an OPEN of an alive gid replaces it (a
+ *     restart).  A CLOSE leaves the gid as rafting_group_close would; a CLOSE of a closed gid changes nothing but the tags.
+ *   Tags: both kinds free every tag of the gid's F lanes in the compact path's in-flight table, if that table exists.
+ *   Pump contract: incarnations restart at 1 (RaftMember.java:20-26), so the engine cannot tell a reply to the old life from
+ *     one to the new.  After an edit of gid g the caller must not put a reply to an RPC planned before the edit into any later
+ *     step, dense or compact: it drops those RPCs from its pending table, as the reference drops the callbacks of a closed
+ *     context.
+ *   Validation: every record is checked on the host before anything is enqueued (RAFTING_E_INVAL / RAFTING_E_CAPACITY, with
+ *     nothing enqueued): gid < max_groups and gids strictly increasing within the call, a known kind, every check
+ *     group_open_bulk makes on init, and for n_runs > 0 every check load_runs makes, against the record's own init.
+ *     n == 0 is a no-op.
+ *   Buffers: `edits` may be reused as soon as the call returns.  The records travel from pinned staging of the engine's own,
+ *     reused under an event: the call blocks only to reuse a staging buffer whose edit has not yet run, or to grow one. */
+enum { RAFTING_EDIT_OPEN = 1, RAFTING_EDIT_CLOSE = 2 };
+typedef struct rafting_group_edit {
+    uint32_t gid, kind;
+    rafting_group_init_t init;                 /* OPEN: exactly what rafting_group_open takes; CLOSE: ignored */
+    uint32_t n_runs, _pad;                     /* OPEN: 0 = the single run init describes (rafting_group_open);
+                                                  1..RAFTING_TERM_RUNS = runs[] as rafting_group_load_runs takes them */
+    rafting_i64x2_t runs[RAFTING_TERM_RUNS];   /* (first index, term), oldest first */
+} rafting_group_edit_t;
+int rafting_group_edit_begin(rafting_engine_t* e, uint32_t n, const rafting_group_edit_t* edits /* host */);
+
 /* host path: fill lease->in (pinned), call step; H2D + kernels + D2H happen inside the call */
 int rafting_lease(rafting_engine_t* e, uint32_t rows, uint32_t n_active, uint32_t ent_count,
                   rafting_lease_t* out);

@@ -117,6 +117,12 @@ GROUP_INIT_DTYPE = np.dtype([
 ])
 assert GROUP_INIT_DTYPE.itemsize == C.sizeof(GroupInit)
 
+EDIT_OPEN = 1
+EDIT_CLOSE = 2
+# rafting_group_edit_t: one record of rafting_group_edit_begin
+GROUP_EDIT = np.dtype([("gid", "<u4"), ("kind", "<u4"), ("init", GROUP_INIT_DTYPE), ("n_runs", "<u4"), ("_pad", "<u4"),
+                       ("runs", I64X2, (TERM_RUNS,))])
+
 
 class FollowerState(C.Structure):
     _fields_ = [

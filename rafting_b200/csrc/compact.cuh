@@ -354,6 +354,7 @@ struct CompactState {
     uint32_t* bits = nullptr;               // [G * F] tags in use
 };
 static void compact_release(rafting_engine* e) { delete e->compact; e->compact = nullptr; }   // the buffers are in dev_allocs
+static uint32_t* compact_bits(rafting_engine* e) { return e->compact ? e->compact->bits : nullptr; }
 static int compact_state(rafting_engine* e) {
     if (e->compact) return RAFTING_OK;
     CompactState* c = new CompactState();

@@ -95,6 +95,7 @@ struct rafting_engine {
     bool alloc_state = true;           // what dalloc marks new allocations as
     struct CompactState* compact = nullptr;   // in-flight table of the compact host path (compact.cuh), created on first use
     struct DuePath* due = nullptr;             // query slots of rafting_timers_due_begin (timers.cuh), created on first use
+    struct EditPath* edit = nullptr;           // staging of rafting_group_edit_begin, created on first use
 };
 
 template <typename T>
@@ -114,7 +115,9 @@ static void rafting_hostpath_release(rafting_engine* e);
 static void seglog_release(rafting_engine* e);
 static void compact_release(rafting_engine* e);
 static void due_release(rafting_engine* e);
+static void edit_release(rafting_engine* e);
 static int compact_state(rafting_engine* e);
+static uint32_t* compact_bits(rafting_engine* e);
 static int quiesce_for_table_edit(rafting_engine* e, const char* who);
 extern "C" uint32_t rafting_abi_version(void) { return RAFTING_ABI_VERSION; }
 extern "C" const char* rafting_last_error(void) { return g_err; }
@@ -178,6 +181,7 @@ extern "C" int rafting_engine_destroy(rafting_engine_t* e) {
     for (void* p : e->shadow) if (p) cudaFree(p);
     compact_release(e);
     due_release(e);
+    edit_release(e);
     rafting_hostpath_release(e);
     seglog_release(e);
     if (e->ev_seg) cudaEventDestroy(e->ev_seg);
@@ -186,10 +190,44 @@ extern "C" int rafting_engine_destroy(rafting_engine_t* e) {
     return RAFTING_OK;
 }
 
+// One group's rows as an open writes them: g_meta, g_term, g_commit, g_lo, g_hi, g_timer, g_epoch and the g_runs planes (newest
+// run first); g_elect, g_err and the l_* planes of its lanes are zero.  rafting_group_open_bulk copies them column by column,
+// rafting_group_edit_begin ships them to group_edit_kernel as records, so the two paths compute them in one place.
+struct EditRow { uint32_t gid, kind; uint64_t meta; int64_t term, commit, lo, hi, timer; i64x2 epoch; i64x2 runs[KRUNS]; };
+
 // ContextManager.buildContext + RaftContext.initialize (RaftContext.java:91-113): the group starts
 // as Follower(restore.term, restore.ballot) — first RaftMember construction (incarnation 1) — with
 // an armed election timer: resetTimer with a null ticket gives max(0 + 1, now + timeout)
 // (RaftRoutine.java:95-107).
+static int open_row(const rafting_engine* e, uint32_t gid, const rafting_group_init_t& g, EditRow& r) {
+    const bool has = g.last_index >= g.first_index;
+    if (has && g.first_index != g.epoch_index && g.first_index != g.epoch_index + 1)
+        return fail(RAFTING_E_INVAL, "group %u: first_index must be epoch_index or epoch_index+1", gid);
+    if (g.ballot < -1 || g.ballot >= (int)e->cfg.replicas) return fail(RAFTING_E_INVAL, "group %u: bad ballot", gid);
+    memset(&r, 0, sizeof(r));
+    r.gid = gid; r.kind = RAFTING_EDIT_OPEN;
+    const uint32_t word = RAFTING_ROLE_FOLLOWER | W_ALIVE | ((uint32_t)(g.ballot + 1) << W_BALLOT_SH) | ((has ? 1u : 0u) << W_NRUNS_SH);
+    r.meta = (uint64_t)word | (1ull << 32);
+    r.term = g.term; r.commit = g.commit_index;
+    r.lo = has ? g.first_index : 1; r.hi = has ? g.last_index : 0;
+    const int64_t draw = g.rand_ms != 0 ? g.rand_ms : rafting_draw(e->cfg.timer_seed, gid, 1, e->cfg.election_ms);
+    const int64_t b = (INT64_MAX - draw < g.now_ms) ? INT64_MAX : g.now_ms + draw;
+    r.timer = b > 1 ? b : 1;
+    r.epoch.x = g.epoch_index; r.epoch.y = g.epoch_term;
+    r.runs[0].x = has ? g.first_index : 0; r.runs[0].y = has ? g.last_term : 0;
+    return RAFTING_OK;
+}
+// rafting_group_load_runs' checks of 1..KRUNS runs (oldest first) against a stored log [lo, hi] whose last term is last_term;
+// out gets them newest first, as g_runs keeps them
+static int runs_rows(int64_t lo, int64_t hi, int64_t last_term, const rafting_i64x2_t* runs, uint32_t n, i64x2* out) {
+    if (runs[0].x != lo || runs[n - 1].y != last_term) return fail(RAFTING_E_INVAL, "runs do not match the opened log (first index / last term)");
+    for (uint32_t k = 1; k < n; k++)
+        if (runs[k].x <= runs[k - 1].x || runs[k].x > hi || runs[k].y == runs[k - 1].y) return fail(RAFTING_E_INVAL, "runs must start at increasing indices inside the log and change term");
+    for (uint32_t k = 0; k < n; k++) { out[k].x = runs[n - 1 - k].x; out[k].y = runs[n - 1 - k].y; }
+    return RAFTING_OK;
+}
+static uint64_t with_nruns(uint64_t m, uint32_t n) { return (m & ~((uint64_t)0xf << W_NRUNS_SH)) | ((uint64_t)n << W_NRUNS_SH); }
+
 extern "C" int rafting_group_open_bulk(rafting_engine_t* e, uint32_t first, uint32_t count, const rafting_group_init_t* in) {
     if (!e || !in) return fail(RAFTING_E_INVAL, "null argument");
     if ((uint64_t)first + count > e->G) return fail(RAFTING_E_CAPACITY, "gid range beyond max_groups");
@@ -203,21 +241,10 @@ extern "C" int rafting_group_open_bulk(rafting_engine_t* e, uint32_t first, uint
     std::vector<uint64_t> meta(count); std::vector<int64_t> term(count), commit(count), lo(count), hi(count), timer(count);
     std::vector<i64x2> epoch(count), elect(count), run0(count); std::vector<uint32_t> err(count, 0);
     for (uint32_t k = 0; k < count; k++) {
-        const rafting_group_init_t& g = in[k];
-        const bool has = g.last_index >= g.first_index;
-        if (has && g.first_index != g.epoch_index && g.first_index != g.epoch_index + 1)
-            return fail(RAFTING_E_INVAL, "group %u: first_index must be epoch_index or epoch_index+1", first + k);
-        if (g.ballot < -1 || g.ballot >= (int)e->cfg.replicas) return fail(RAFTING_E_INVAL, "group %u: bad ballot", first + k);
-        uint32_t word = RAFTING_ROLE_FOLLOWER | W_ALIVE | ((uint32_t)(g.ballot + 1) << W_BALLOT_SH) | ((has ? 1u : 0u) << W_NRUNS_SH);
-        meta[k] = (uint64_t)word | (1ull << 32);
-        term[k] = g.term; commit[k] = g.commit_index;
-        lo[k] = has ? g.first_index : 1; hi[k] = has ? g.last_index : 0;
-        int64_t draw = g.rand_ms != 0 ? g.rand_ms : rafting_draw(e->cfg.timer_seed, first + k, 1, e->cfg.election_ms);
-        int64_t b = (INT64_MAX - draw < g.now_ms) ? INT64_MAX : g.now_ms + draw;
-        timer[k] = b > 1 ? b : 1;
-        epoch[k].x = g.epoch_index; epoch[k].y = g.epoch_term;
-        elect[k].x = 0; elect[k].y = 0;
-        run0[k].x = has ? g.first_index : 0; run0[k].y = has ? g.last_term : 0;
+        EditRow r;
+        if (int rc = open_row(e, first + k, in[k], r)) return rc;
+        meta[k] = r.meta; term[k] = r.term; commit[k] = r.commit; lo[k] = r.lo; hi[k] = r.hi; timer[k] = r.timer;
+        epoch[k] = r.epoch; elect[k].x = 0; elect[k].y = 0; run0[k] = r.runs[0];
     }
     Tables& T = e->T;
     CU(cudaMemcpy(T.g_meta + first, meta.data(), count * 8, cudaMemcpyHostToDevice));
@@ -251,14 +278,10 @@ extern "C" int rafting_group_load_runs(rafting_engine_t* e, uint32_t gid, const 
     CU(cudaMemcpy(&hi, e->T.g_hi + gid, 8, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(&newest, e->T.g_runs + gid, 16, cudaMemcpyDeviceToHost));
     if (!(m & W_ALIVE) || ((uint32_t)(m >> W_NRUNS_SH) & 0xf) != 1 || hi < lo) return fail(RAFTING_E_INVAL, "group %u is not a freshly opened group with a stored log", gid);
-    if (runs[0].x != lo || runs[n - 1].y != newest.y) return fail(RAFTING_E_INVAL, "runs do not match the opened log (first index / last term)");
-    for (uint32_t k = 1; k < n; k++)
-        if (runs[k].x <= runs[k - 1].x || runs[k].x > hi || runs[k].y == runs[k - 1].y) return fail(RAFTING_E_INVAL, "runs must start at increasing indices inside the log and change term");
-    for (uint32_t k = 0; k < n; k++) {                                       // newest run first in the table
-        i64x2 v; v.x = runs[n - 1 - k].x; v.y = runs[n - 1 - k].y;
-        CU(cudaMemcpy(e->T.g_runs + (size_t)k * e->G + gid, &v, 16, cudaMemcpyHostToDevice));
-    }
-    m = (m & ~((uint64_t)0xf << W_NRUNS_SH)) | ((uint64_t)n << W_NRUNS_SH);
+    i64x2 rows[KRUNS];
+    if (int rc = runs_rows(lo, hi, newest.y, runs, n, rows)) return rc;
+    for (uint32_t k = 0; k < n; k++) CU(cudaMemcpy(e->T.g_runs + (size_t)k * e->G + gid, &rows[k], 16, cudaMemcpyHostToDevice));   // newest run first in the table
+    m = with_nruns(m, n);
     CU(cudaMemcpy(e->T.g_meta + gid, &m, 8, cudaMemcpyHostToDevice));
     return RAFTING_OK;
 }
@@ -753,6 +776,86 @@ extern "C" int rafting_step(rafting_engine_t* e, rafting_lease_t* L) {
     int rc = rafting_step_begin(e, L);
     if (rc) return rc;
     return rafting_step_wait(e, L);
+}
+
+// ---------------------------------------------------------------------------------------------
+// group edits in step-stream order (rafting_group_edit_begin): the records' rows are built and checked on the host by the
+// functions the synchronous calls use, travel up in one copy on the step stream, and one kernel writes them, so they take
+// effect between the steps begun before the call and those begun after it.
+// ---------------------------------------------------------------------------------------------
+// one thread per record; the gids of a call are distinct, so no two threads touch the same row
+__global__ void __launch_bounds__(256) group_edit_kernel(Tables T, const EditRow* __restrict__ rows, uint32_t n, uint32_t* __restrict__ bits) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const EditRow& r = rows[k];
+    const size_t g = r.gid, F = T.F;
+    if (r.kind == RAFTING_EDIT_CLOSE) {
+        T.g_meta[g] &= ~(uint64_t)W_ALIVE;
+    } else {
+        const i64x2 z = {0, 0};
+        T.g_meta[g] = r.meta; T.g_term[g] = r.term; T.g_commit[g] = r.commit; T.g_lo[g] = r.lo; T.g_hi[g] = r.hi;
+        T.g_timer[g] = r.timer; T.g_epoch[g] = r.epoch; T.g_elect[g] = z; T.g_err[g] = 0;
+        for (int q = 0; q < KRUNS; q++) T.g_runs[(size_t)q * T.G + g] = r.runs[q];
+        for (size_t f = 0; f < F; f++) {
+            T.l_nm[g * F + f] = z; T.l_es[g * F + f] = z; T.l_fr[g * F + f] = z; T.l_cnt[g * F + f] = make_int4(0, 0, 0, 0);
+        }
+    }
+    if (bits)                                      // the compact path's in-flight table: the old life's tags are free again
+        for (size_t f = 0; f < F; f++) bits[g * F + f] = 0;
+}
+
+// Pinned blocks the records travel from, used in turn, each reused once the event recorded behind its edit has fired, and one
+// device block the copies land in: every copy and launch is on the step stream, so the next copy cannot overtake a launch.
+constexpr int EDIT_STAGES = RAFTING_HOST_SLOTS;
+struct EditPath { Blk host[EDIT_STAGES]; cudaEvent_t ev[EDIT_STAGES] = {}; Blk dev; uint32_t next = 0; };
+static void edit_release(rafting_engine* e) {
+    if (!e->edit) return;
+    for (int k = 0; k < EDIT_STAGES; k++) { blk_free(e->edit->host[k], true); if (e->edit->ev[k]) cudaEventDestroy(e->edit->ev[k]); }
+    blk_free(e->edit->dev, false);
+    delete e->edit; e->edit = nullptr;
+}
+static int edit_row(const rafting_engine* e, uint32_t k, const rafting_group_edit_t& d, uint32_t prev_gid, EditRow& r) {
+    if (d.gid >= e->G) return fail(RAFTING_E_CAPACITY, "edit %u: gid %u beyond max_groups", k, d.gid);
+    if (k > 0 && d.gid <= prev_gid) return fail(RAFTING_E_INVAL, "edit %u: gid %u after gid %u (gids must increase strictly)", k, d.gid, prev_gid);
+    if (d.kind == RAFTING_EDIT_CLOSE) { memset(&r, 0, sizeof(r)); r.gid = d.gid; r.kind = d.kind; return RAFTING_OK; }
+    if (d.kind != RAFTING_EDIT_OPEN) return fail(RAFTING_E_INVAL, "edit %u: unknown kind %u", k, d.kind);
+    if (int rc = open_row(e, d.gid, d.init, r)) return rc;
+    if (d.n_runs == 0) return RAFTING_OK;
+    if (d.n_runs > (uint32_t)KRUNS) return fail(RAFTING_E_CAPACITY, "edit %u: %u term runs: the engine keeps at most %d per group", k, d.n_runs, KRUNS);
+    if (r.hi < r.lo) return fail(RAFTING_E_INVAL, "edit %u: group %u has term runs but no stored log", k, d.gid);
+    if (int rc = runs_rows(r.lo, r.hi, d.init.last_term, d.runs, d.n_runs, r.runs)) return rc;
+    r.meta = with_nruns(r.meta, d.n_runs);
+    return RAFTING_OK;
+}
+extern "C" int rafting_group_edit_begin(rafting_engine_t* e, uint32_t n, const rafting_group_edit_t* edits) {
+    if (!e) return fail(RAFTING_E_INVAL, "null argument");
+    if (n == 0) return RAFTING_OK;
+    if (!edits) return fail(RAFTING_E_INVAL, "null argument");
+    if (n > e->G) return fail(RAFTING_E_CAPACITY, "%u edits: more than max_groups", n);
+    CU(cudaSetDevice(e->cfg.device));
+    if (!e->edit) {
+        e->edit = new EditPath();
+        for (int k = 0; k < EDIT_STAGES; k++) CU(cudaEventCreateWithFlags(&e->edit->ev[k], cudaEventDisableTiming));
+    }
+    EditPath& P = *e->edit;
+    const uint32_t st = P.next;
+    const size_t bytes = (size_t)n * sizeof(EditRow);
+    CU(cudaEventSynchronize(P.ev[st]));                     // the stage's previous edit has run (a fresh event counts as fired)
+    int rc;
+    if ((rc = blk_reserve(P.host[st], bytes, true))) return rc;
+    EditRow* rows = (EditRow*)P.host[st].p;
+    for (uint32_t k = 0; k < n; k++)
+        if ((rc = edit_row(e, k, edits[k], k ? edits[k - 1].gid : 0, rows[k]))) return rc;
+    if (bytes > P.dev.cap) {                                 // growing frees the block an earlier edit may still read
+        CU(cudaStreamSynchronize(e->stream));
+        if ((rc = blk_reserve(P.dev, bytes, false))) return rc;
+    }
+    CU(cudaMemcpyAsync(P.dev.p, rows, bytes, cudaMemcpyHostToDevice, e->stream));
+    group_edit_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(e->T, (const EditRow*)P.dev.p, n, compact_bits(e));
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(P.ev[st], e->stream));
+    P.next = (st + 1) % EDIT_STAGES;
+    return RAFTING_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

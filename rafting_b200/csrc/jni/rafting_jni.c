@@ -99,6 +99,10 @@ JNIEXPORT void JNICALL FN(groupOpenBulk)(JNIEnv* env, jclass k, jlong h, jint fi
 JNIEXPORT void JNICALL FN(groupLoadRuns)(JNIEnv* env, jclass k, jlong h, jint gid, jobject runs, jint n) {
     CHECK(rafting_group_load_runs(ENG(h), (uint32_t)gid, (const rafting_i64x2_t*)BUF(runs), (uint32_t)n));
 }
+/* opens, restarts and closes as rafting_group_edit_t records, in step-stream order while steps are in flight (INTEGRATION.md §4) */
+JNIEXPORT void JNICALL FN(groupEditBegin)(JNIEnv* env, jclass k, jlong h, jobject edits, jint n) {
+    CHECK(rafting_group_edit_begin(ENG(h), (uint32_t)n, (const rafting_group_edit_t*)BUF(edits)));
+}
 JNIEXPORT void JNICALL FN(leaseRelease)(JNIEnv* env, jclass k, jlong h, jobject leaseBuf) {
     CHECK(rafting_lease_release(ENG(h), (rafting_lease_t*)BUF(leaseBuf)));
 }

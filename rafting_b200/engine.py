@@ -32,7 +32,7 @@ STATUS = {0: "OK", -1: "E_INVAL", -2: "E_NOMEM", -3: "E_CUDA", -4: "E_CLOSED", -
 
 EXPORTS = [
     "rafting_abi_version", "rafting_last_error", "rafting_engine_create", "rafting_engine_destroy",
-    "rafting_group_open", "rafting_group_open_bulk", "rafting_group_load_runs", "rafting_group_close", "rafting_lease", "rafting_lease_ex", "rafting_lease_release", "rafting_step",
+    "rafting_group_open", "rafting_group_open_bulk", "rafting_group_load_runs", "rafting_group_close", "rafting_group_edit_begin", "rafting_lease", "rafting_lease_ex", "rafting_lease_release", "rafting_step",
     "rafting_step_begin", "rafting_step_wait", "rafting_step_device", "rafting_state_export",
     "rafting_state_export_bulk", "rafting_state_digest", "rafting_log_term", "rafting_commit_slice",
     "rafting_comm_init", "rafting_comm_init_all", "rafting_comm_unique_id", "rafting_allgather_commit", "rafting_allgather_commit_from",
@@ -72,6 +72,7 @@ def lib():
         L.rafting_group_open_bulk.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
         L.rafting_group_close.argtypes = [C.c_void_p, C.c_uint32]
         L.rafting_group_load_runs.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+        L.rafting_group_edit_begin.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
         L.rafting_lease.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(abi.LeaseC)]
         L.rafting_lease_ex.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(abi.LeaseC)]
         L.rafting_lease_release.argtypes = [C.c_void_p, C.POINTER(abi.LeaseC)]
@@ -158,6 +159,36 @@ def _np_view(ptr: int, dtype, shape):
     return np.frombuffer(buf, dtype=dt, count=n).reshape(shape)
 
 
+# rafting_group_init_t of a fresh, empty group: what open_group and edit_open fill in for the keywords they are not given
+_INIT_DEFAULTS = dict(term=0, ballot=-1, epoch_index=0, epoch_term=0, first_index=1, last_index=0, last_term=0,
+                      commit_index=0, now_ms=0, rand_ms=1000)
+
+
+def edit_open(gid: int, runs=None, **kw) -> np.ndarray:
+    """One OPEN record for Engine.group_edit_begin: the keywords of open_group, plus runs = [(first index, term), ...]
+    oldest first as load_runs takes them (None: the single run the init describes)."""
+    r = np.zeros((), dtype=abi.GROUP_EDIT)
+    r["gid"], r["kind"] = gid, abi.EDIT_OPEN
+    d = dict(_INIT_DEFAULTS)
+    d.update(kw)
+    for k, v in d.items():
+        r["init"][k] = v
+    if runs is not None:
+        a = np.array(runs, dtype=np.int64).reshape(-1, 2)
+        if len(a) > abi.TERM_RUNS:
+            raise ValueError(f"{len(a)} term runs: a record holds at most {abi.TERM_RUNS}")
+        r["n_runs"] = len(a)
+        r["runs"][:len(a)] = np.rec.fromarrays(a.T, dtype=abi.I64X2)
+    return r
+
+
+def edit_close(gid: int) -> np.ndarray:
+    """One CLOSE record for Engine.group_edit_begin."""
+    r = np.zeros((), dtype=abi.GROUP_EDIT)
+    r["gid"], r["kind"] = gid, abi.EDIT_CLOSE
+    return r
+
+
 class Engine:
     def __init__(self, cfg: abi.Cfg):
         self.cfg = cfg
@@ -181,8 +212,7 @@ class Engine:
     # ---- lifecycle -------------------------------------------------------------------------
     def open_group(self, gid: int, **kw):
         gi = abi.GroupInit()
-        d = dict(term=0, ballot=-1, epoch_index=0, epoch_term=0, first_index=1, last_index=0, last_term=0,
-                 commit_index=0, now_ms=0, rand_ms=1000)
+        d = dict(_INIT_DEFAULTS)
         d.update(kw)
         for k, v in d.items():
             setattr(gi, k, v)
@@ -199,6 +229,13 @@ class Engine:
 
     def close_group(self, gid: int):
         _check(lib().rafting_group_close(self._h, gid), "rafting_group_close")
+
+    def group_edit_begin(self, edits):
+        """Enqueues opens, restarts and closes (abi.GROUP_EDIT records, built by edit_open / edit_close, gids increasing) on
+        the step stream, behind every step begun so far, without draining it.  The caller drops its pending RPCs of the
+        edited gids: their replies must not reach a later step."""
+        a = np.ascontiguousarray(np.asarray(edits, dtype=abi.GROUP_EDIT).reshape(-1))
+        _check(lib().rafting_group_edit_begin(self._h, len(a), a.ctypes.data), "rafting_group_edit_begin")
 
     # ---- host path: lease -> fill pinned columns -> step (H2D + kernel + D2H inside) ----------
     def lease(self, rows: int, n_active: int = 0, ent_count: int = 0, flags: int = 0) -> "Lease":

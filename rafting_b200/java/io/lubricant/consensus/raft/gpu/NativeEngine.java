@@ -25,6 +25,7 @@ final class NativeEngine {
     // ---- round 2 ----
     static native void groupOpenBulk(long h, int first, int count, ByteBuffer inits);            // rafting_group_open_bulk
     static native void groupLoadRuns(long h, int gid, ByteBuffer runs, int n);                   // rafting_group_load_runs (restart, §4)
+    static native void groupEditBegin(long h, ByteBuffer edits, int n);                          // rafting_group_edit_begin: opens / restarts / closes between steps
     static native void leaseRelease(long h, ByteBuffer leaseStruct);                             // rafting_lease_release
     static native void stepBeginHost(long h, int slot, ByteBuffer inboxStruct, ByteBuffer outboxStruct);   // rafting_step_begin_host: Netty's pinned receive pool
     static native void stepWaitSlot(long h, int slot);                                           // rafting_step_wait_slot
