@@ -781,6 +781,42 @@ int rafting_log_gather(rafting_engine_t* e, uint32_t n_ranges, const uint32_t* g
 /* garbage collection behind RaftLog.flush (RocksLog.java:228-242): drops the index entries below each group's lowest
    stored key and frees cold (pinned host) segments that hold no live record any more */
 int rafting_log_trim  (rafting_engine_t* e, uint32_t first_gid, uint32_t count, uint64_t* dropped_entries, uint64_t* freed_cold_bytes);
+/* PAYLOADS OF A COMPACT STEP'S PLANS, gathered on the device: what rafting_log_gather returns for the step's AppendEntries
+ * ranges, without decoding plan_c words or escape records on the host.
+ *   * Which plans: those of the compact step last waited for in `slot`, whatever its shape (whole shard, active, sweep or due;
+ *     flags 0, 1, 4 or 5; escaped plans included); the precondition of rafting_step_fetch_dense.  A plan of kind AE with entry
+ *     count c > 0 asks for indices plan_pp.x + 1 ... plan_pp.x + c of its group; heartbeats without entries, IS, SKIP_INFLIGHT
+ *     and UNAVAILABLE plans ask for nothing, and so does a step with no op and no sweep row (it has no plan columns).  Plans are
+ *     walked in lane-slot order (row * n + position) * F + lane; positions map to gids through the step's list, a due step's
+ *     device-chosen tail included.
+ *   * refs_out: one record per asked-for entry, plan after plan in that order: exactly the gid, index, term and len that
+ *     rafting_log_gather returns for the same ranges in the same order (len 0xffffffff: never appended).
+ *     plans_out: one record per plan with entries (its lane slot, its first ref, its count).
+ *     blob_out: the payloads at blob_off, 16-byte aligned; entries served on the device first, in ref order, then the entries
+ *     the host serves.
+ *   * Semantics: the payloads are what rafting_log_gather over those ranges returns at the point in the entry buffer's stream
+ *     where the begin is enqueued.  Visibility stays the caller's, as for rafting_log_gather.
+ *   * Ordering: the work runs on the entry buffer's stream, behind every rafting_log_append made before the begin (the payloads
+ *     of the SUBMITs that created the step's entries included); the step stream never waits for it.  rafting_log_append,
+ *     rafting_log_trim and rafting_log_store_open return RAFTING_E_BUSY while a gather is not waited for.
+ *   * Host-served entries: an entry the device ring does not hold (the ring slot caches a newer index, the record is in the
+ *     pinned cold tier or the entry file, or it was never appended) goes to a miss list, which the wait serves through the host
+ *     index; host work is proportional to misses.  *host_served is their number.
+ *   * Capacity: nothing past refs_cap, plans_cap or blob_cap is written; when one is exceeded the wait returns
+ *     RAFTING_E_CAPACITY with the sizes needed in *n_refs, *bytes, *n_plans.  The slot's plans stay resident: begin again.
+ *   * Slot lifetime: a slot holds at most one gather (a second begin is RAFTING_E_BUSY); while it is not waited for, every step
+ *     begin on the slot returns RAFTING_E_BUSY with nothing enqueued.  A begin without a finished compact step in the slot, or
+ *     without rafting_log_config, is RAFTING_E_INVAL.
+ *   * Output memory: pinned or registered outputs (blob_out 16-byte aligned) are written by the device directly, so only the
+ *     gathered bytes cross PCIe; any other host memory goes through pinned staging of the slot, copied at the wait.  Outputs
+ *     stay valid until the wait; nothing synchronises the host between begin and wait. */
+typedef struct rafting_plan_ref { uint32_t slot, first, count, _pad; } rafting_plan_ref_t;   /* lane slot, first ref, refs */
+int rafting_log_gather_step_begin(rafting_engine_t* e, uint32_t slot /* 0..3 */,
+                                  rafting_entry_ref_t* refs_out, uint32_t refs_cap,
+                                  void* blob_out, size_t blob_cap,
+                                  rafting_plan_ref_t* plans_out, uint32_t plans_cap);
+int rafting_log_gather_step_wait (rafting_engine_t* e, uint32_t slot,
+                                  uint32_t* n_refs, size_t* bytes, uint32_t* n_plans, uint32_t* host_served);
 int rafting_log_stats (rafting_engine_t* e, uint64_t* out /* appended, head, spilled_bytes, hbm_hits, cold_hits, indexed,
                                                               last gather kernels ns, last gather bytes, trimmed entries,
                                                               cold bytes freed, spills skipped (dead segments) */, uint32_t n);

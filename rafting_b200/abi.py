@@ -122,6 +122,8 @@ EDIT_CLOSE = 2
 # rafting_group_edit_t: one record of rafting_group_edit_begin
 GROUP_EDIT = np.dtype([("gid", "<u4"), ("kind", "<u4"), ("init", GROUP_INIT_DTYPE), ("n_runs", "<u4"), ("_pad", "<u4"),
                        ("runs", I64X2, (TERM_RUNS,))])
+# rafting_plan_ref_t: one plan with entries of rafting_log_gather_step_begin (lane slot, first ref, number of refs)
+PLAN_REF = np.dtype([("slot", "<u4"), ("first", "<u4"), ("count", "<u4"), ("_pad", "<u4")])
 
 
 class FollowerState(C.Structure):

@@ -401,3 +401,27 @@ def decode_outbox(co: CompactOutbox, G: int | None = None, elections: bool = Fal
             rr, i = divmod(slot, n)
             o.rep_meta[rr, i] = r["meta"]; o.rep_term[rr, i] = r["a"]
     return o
+
+
+def ae_ranges(co: CompactOutbox) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The AppendEntries ranges a compact outbox asks payloads for, as a pump decodes them for rafting_log_gather: plans of
+    kind AE (1, or 7 under RAFTING_COMPACT_PREV_TERM, or an escaped AE) with entries, in lane-slot order (row * n + position)
+    * F + lane.  -> (lane slots, gids, first indices, counts); rafting_log_gather_step_begin walks the same plans on the device."""
+    w = co.plan_c.reshape(-1)
+    kind, esc = w & 7, (w >> 4) & 1
+    first = np.zeros(len(w), np.int64)
+    count = np.where(esc == 0, (w >> 11) & 63, 0).astype(np.int64)
+    ae = (esc == 0) & ((kind == 1) | (kind == abi.CPLAN_AE_PREV_TERM))
+    pos = (np.arange(len(w)) // co.F) % co.n
+    first[ae] = co.last_entry["x"][pos[ae]] - ((w[ae] >> 17) & 255) + 1
+    rec = co.esc[:min(int(co.counts[0]), co.esc_cap)]
+    rec = rec[(rec["kind"] == abi.CESC_PLAN) & (rec["slot"] < len(w))]
+    ek = rec["meta"] & 0xF
+    ec = (rec["meta"] >> 16) & 0xFFFF
+    s = rec["slot"].astype(np.int64)
+    ae[s] = ek == abi.PLAN_AE
+    count[s] = ec.astype(np.int64)
+    first[s] = rec["a"] + 1
+    t = np.flatnonzero(ae & (count > 0))
+    gids = pos[t] if co.gids is None else co.gids[pos[t]].astype(np.int64)
+    return t, gids, first[t], count[t]

@@ -517,6 +517,7 @@ static int compact_check(rafting_engine_t* e, uint32_t slot, uint32_t flags, uin
     const Slot& S = hp(e)->slot[slot];
     if (S.leased) return fail(RAFTING_E_BUSY, "slot %u is held by an outstanding lease", slot);
     if (S.inflight) return fail(RAFTING_E_BUSY, "slot %u has a step in flight", slot);
+    if (S.gathering) return fail(RAFTING_E_BUSY, "slot %u: the gather of its plans has not been waited for", slot);
     p.list = p.gids != nullptr || due != nullptr;
     const size_t rows = in->rows, n = p.list ? n_active : e->G, F = e->F;
     p.rows = rows; p.n = n; p.n_listed = due ? due->n_host : n;
@@ -689,7 +690,7 @@ static int compact_begin(rafting_engine_t* e, uint32_t slot, const rafting_cinbo
     CU(cudaEventRecord(S.ev_done, H->s_d2h));
     S.compact_step = true; S.c_host = *out; S.c_counts_pinned = (uint32_t*)counts.h; S.c_esc_dev = S.cout.p + LC.esc_out;
     S.c_tail_user = due ? due->tail_out : nullptr; S.c_tail_n = due ? due->cap : 0;
-    S.dev_out = p.dout; S.rows_ = rows; S.n_ = n;
+    S.dev_out = p.dout; S.rows_ = rows; S.n_ = n; S.c_gids = p.list ? p.din.gids : nullptr;
     S.inflight = true;
     return RAFTING_OK;
 }

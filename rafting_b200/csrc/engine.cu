@@ -525,6 +525,9 @@ struct Slot {
     uint32_t lease_gen = 0;
     // of the step in flight (for the sparse columns fetched at wait time)
     rafting_outbox_t host_out; rafting_outbox_t dev_out; size_t rows_ = 0, n_ = 0; const uint32_t* flags_host = nullptr;
+    const uint32_t* c_gids = nullptr;         // device list of the compact step (null: whole shard), due tail included
+    struct StepGather* gather = nullptr;      // rafting_log_gather_step_begin (seglog.cuh), created on first use
+    bool gathering = false;                   // a gather of this slot's plans has not been waited for: no step may reuse the slot
 };
 struct HostPath {
     Slot slot[RAFTING_HOST_SLOTS];
@@ -532,6 +535,7 @@ struct HostPath {
     bool ready = false;
 };
 static HostPath* hp(rafting_engine* e) { if (!e->host) e->host = new HostPath(); return e->host; }
+static void step_gather_release(Slot& s);
 
 // Host-side edits of the tables (group open / close / load_runs) must not interleave with step kernels: RAFTING_E_BUSY
 // while a host-path step has been begun and not waited for, then the step stream is drained.
@@ -566,6 +570,7 @@ static void hostpath_free(rafting_engine* e) {
         if (s.ev_kernel) cudaEventDestroy(s.ev_kernel);
         if (s.ev_done) cudaEventDestroy(s.ev_done);
         if (s.h_flags) cudaFreeHost(s.h_flags);
+        step_gather_release(s);
     }
     if (H->s_h2d) cudaStreamDestroy(H->s_h2d);
     if (H->s_d2h) cudaStreamDestroy(H->s_d2h);
@@ -595,6 +600,7 @@ static int issue_copies(std::vector<CopyItem>& v, bool to_device, cudaStream_t s
 static int step_enqueue(rafting_engine* e, uint32_t slot, const rafting_inbox_t* in, const rafting_outbox_t* out) {
     HostPath* H = hp(e); Slot& S = H->slot[slot];
     if (S.inflight) return fail(RAFTING_E_BUSY, "slot %u has a step in flight", slot);
+    if (S.gathering) return fail(RAFTING_E_BUSY, "slot %u: the gather of its plans has not been waited for", slot);
     const size_t rows = in->rows, F = e->F, G = e->G;
     const bool list = in->gids != nullptr;
     const size_t n = list ? in->n_active : G;

@@ -202,6 +202,26 @@ JNIEXPORT jint JNICALL FN(logGather)(JNIEnv* env, jclass k, jlong h, jint nRange
                              (rafting_entry_ref_t*)BUF(refsOut), (uint32_t)refsCap, BUF(blobOut), (size_t)blobCap, &n, &bytes));
     return (jint)n;
 }
+/* the payloads of the AppendEntries plans of the compact step last waited for in `slot`, gathered on the device (INTEGRATION.md §7) */
+JNIEXPORT void JNICALL FN(logGatherStepBegin)(JNIEnv* env, jclass k, jlong h, jint slot, jobject refsOut, jint refsCap, jobject blobOut,
+                                              jlong blobCap, jobject plansOut, jint plansCap) {
+    CHECK(rafting_log_gather_step_begin(ENG(h), (uint32_t)slot, (rafting_entry_ref_t*)BUF(refsOut), (uint32_t)refsCap, BUF(blobOut),
+                                        (size_t)blobCap, (rafting_plan_ref_t*)BUF(plansOut), (uint32_t)plansCap));
+}
+/* result = {nRefs, bytes, nPlans, hostServed}; they are written before RAFTING_E_CAPACITY is thrown, as the sizes needed */
+JNIEXPORT void JNICALL FN(logGatherStepWait)(JNIEnv* env, jclass k, jlong h, jint slot, jlongArray result) {
+    if (!result || (*env)->GetArrayLength(env, result) < 4) {
+        jclass c = (*env)->FindClass(env, "java/lang/IllegalArgumentException");
+        if (c) (*env)->ThrowNew(env, c, "logGatherStepWait: the result array needs 4 elements {nRefs, bytes, nPlans, hostServed}");
+        return;
+    }
+    uint32_t n = 0, plans = 0, served = 0; size_t bytes = 0;
+    int rc = rafting_log_gather_step_wait(ENG(h), (uint32_t)slot, &n, &bytes, &plans, &served);
+    jlong* r = (*env)->GetLongArrayElements(env, result, NULL);
+    r[0] = (jlong)n; r[1] = (jlong)bytes; r[2] = (jlong)plans; r[3] = (jlong)served;
+    (*env)->ReleaseLongArrayElements(env, result, r, 0);
+    if (rc) throw_status(env, rc);
+}
 JNIEXPORT void JNICALL FN(logTrim)(JNIEnv* env, jclass k, jlong h, jint first, jint count) {
     CHECK(rafting_log_trim(ENG(h), (uint32_t)first, (uint32_t)count, NULL, NULL));
 }

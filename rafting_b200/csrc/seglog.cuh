@@ -34,6 +34,9 @@ static_assert(sizeof(SegHdr) == 32, "segment record header");
 struct HostLoc { uint64_t off; uint32_t len; int64_t term; uint64_t file_off; };      // len == 0xffffffff: absent; file_off: payload offset in the durable file (~0 = none)
 constexpr uint64_t NO_FILE = ~0ull, NO_ARENA = ~0ull;                                  // off == NO_ARENA: recovered from the file, never resident
 struct GroupIdx { int64_t base = 0; std::vector<HostLoc> v; int64_t epoch_index = 0, epoch_term = 0; };     // host index of one group: v[i] <-> index base + i
+// What a group's host index has dropped while the device ring may still name it: indices below `index` (rafting_log_trim, the
+// index window moving up) and records appended before `seq` (the window restarting elsewhere).  The ring serves neither.
+struct Floor { int64_t index; uint64_t seq; };
 
 struct SegLog {
     uint32_t seg_bytes = 0, nseg = 0, K = 0;
@@ -63,6 +66,10 @@ struct SegLog {
     std::vector<uint32_t> seg_live;           // live (indexed, not overwritten, not trimmed) records per logical segment
     uint64_t trimmed = 0, cold_freed_bytes = 0, spills_skipped = 0;
     cudaEvent_t t0 = nullptr, t1 = nullptr;    // device time of the last gather's kernel
+    std::vector<Floor> floor;                 // [G] host copy of d_floor; gids floor_lo..floor_hi changed since the last upload
+    Floor* d_floor = nullptr;
+    uint32_t floor_lo = UINT32_MAX, floor_hi = 0;
+    uint32_t step_gathers = 0;                // rafting_log_gather_step_begin calls not waited for
     float last_gather_kernel_ms = 0; uint64_t last_gather_bytes = 0;
 };
 
@@ -95,6 +102,39 @@ __global__ void seglog_scatter_kernel(const AppendRec* __restrict__ recs, uint32
 
 struct GatherReq { uint32_t gid; uint32_t slot; int64_t index; uint64_t out_off; };   // slot: position in the reply list
 
+// The hit test of the entry buffer: the ring slot of (gid, index) names the newest record published there, and it serves
+// the entry when that record is still in the HBM arena and is exactly (gid, index).  rec: the record, len: its payload bytes.
+__device__ __forceinline__ bool seglog_hit(const unsigned long long* __restrict__ ring, uint32_t K, const uint8_t* __restrict__ arena,
+                                           uint64_t arena_bytes, uint64_t oldest_resident, uint32_t gid, int64_t index,
+                                           const uint8_t*& rec, uint32_t& len) {
+    const unsigned long long loc1 = ring[(size_t)gid * K + ((uint64_t)index & (K - 1))];
+    bool hit = loc1 != 0 && loc1 - 1 >= oldest_resident;
+    len = 0;
+    rec = arena + ((loc1 - 1) % arena_bytes);
+    if (hit) {
+        const int4 h0 = *(const int4*)rec;                       // gid, len, index
+        const long long idx = ((long long)(unsigned)h0.w << 32) | (unsigned)h0.z;
+        hit = (uint32_t)h0.x == gid && idx == index;
+        len = (uint32_t)h0.y;
+    }
+    return hit;
+}
+
+// One requested entry on 8 lanes: *len_out = its length, or 0xffffffff when the ring does not hold it; on a hit the payload
+// goes to out + q.out_off
+__device__ __forceinline__ void seglog_gather_entry(const GatherReq& q, uint32_t sub, const unsigned long long* __restrict__ ring,
+                                                    uint32_t K, const uint8_t* __restrict__ arena, uint64_t arena_bytes,
+                                                    uint64_t oldest_resident, uint32_t* __restrict__ len_out, uint8_t* __restrict__ out) {
+    const uint8_t* rec; uint32_t len;
+    const bool hit = seglog_hit(ring, K, arena, arena_bytes, oldest_resident, q.gid, q.index, rec, len);
+    if (sub == 0) *len_out = hit ? len : 0xffffffffu;
+    if (!hit) return;
+    const int4* src = (const int4*)(rec + sizeof(SegHdr));       // records and payloads are 16-byte aligned
+    int4* dst = (int4*)(out + q.out_off);                        // out_off is 16-byte aligned
+    const uint32_t words = (len + 15) >> 4;
+    for (uint32_t i = sub; i < words; i += 8) dst[i] = src[i];
+}
+
 // 8 lanes per requested entry (4 entries per warp, so four dependent chains ring -> header -> payload are in
 // flight per warp), 16-byte vector copies HBM arena -> contiguous send buffer.  lens[e] = 0xffffffff when the
 // ring does not point at a resident record of exactly (gid, index); the host then serves it from its index.
@@ -105,22 +145,103 @@ __global__ void seglog_gather_kernel(const GatherReq* __restrict__ req, uint32_t
     const uint32_t en = t >> 3, sub = t & 7;
     if (en >= n) return;
     const GatherReq q = req[en];
-    const unsigned long long loc1 = ring[(size_t)q.gid * K + ((uint64_t)q.index & (K - 1))];
-    bool hit = loc1 != 0 && loc1 - 1 >= oldest_resident;
-    uint32_t len = 0;
-    const uint8_t* rec = arena + ((loc1 - 1) % arena_bytes);
-    if (hit) {
-        const int4 h0 = *(const int4*)rec;                       // gid, len, index
-        const long long idx = ((long long)(unsigned)h0.w << 32) | (unsigned)h0.z;
-        hit = (uint32_t)h0.x == q.gid && idx == q.index;
-        len = (uint32_t)h0.y;
+    seglog_gather_entry(q, sub, ring, K, arena, arena_bytes, oldest_resident, lens + en, out);
+}
+
+// ---- the payloads of a compact step's plans (rafting_log_gather_step_begin) ----
+// Four passes on the entry buffer's stream over the step's dense plan columns, which stay resident after its wait:
+//   step_plan_count_kernel   one thread per lane slot: the entries an AE plan asks for, and whether it has any
+//   (cub scan)               -> each plan's first ref and its plan record
+//   step_plan_probe_kernel   one thread per lane slot, over its entries: hit or miss, and the 16-byte-aligned bytes of its hits
+//   (cub scan)               -> each plan's first blob offset, first miss and first gather request
+//   step_plan_emit_kernel    the refs and plan records, one gather request per hit, the miss list
+//   step_gather_copy_kernel  seglog_gather_entry over the requests, whose number only the device knows
+struct GAgg { uint64_t a, b, c; };              // pass 1: (refs, plans, 0); pass 2: (device bytes, misses, hits)
+struct GAggSum { __device__ __forceinline__ GAgg operator()(const GAgg& x, const GAgg& y) const { return GAgg{x.a + y.a, x.b + y.b, x.c + y.c}; } };
+
+struct StepPlansD {                             // the step's dense plan columns; lane slot t stands for position (t / F) % n
+    const uint64_t* plan_meta; const rafting_i64x2_t* plan_pp; const uint32_t* gids; uint32_t n, F, P;
+};
+struct ProbeD {                                 // what seglog_hit reads, and the host index's floors
+    const unsigned long long* ring; uint32_t K; const uint8_t* arena; uint64_t arena_bytes, oldest; const Floor* floor;
+};
+struct StepOutD {
+    rafting_entry_ref_t* refs; uint32_t refs_cap, plans_cap; rafting_plan_ref_t* plans; uint64_t blob_cap;
+    GatherReq* req; uint32_t* miss;
+};
+
+__device__ __forceinline__ uint32_t plan_entries(uint64_t m) { return (m & 0xfu) == RAFTING_PLAN_AE ? (uint32_t)(m >> 16) & 0xffffu : 0u; }
+__device__ __forceinline__ uint32_t plan_gid(const StepPlansD& s, uint32_t t) { const uint32_t i = (t / s.F) % s.n; return s.gids ? s.gids[i] : i; }
+// seglog_hit, minus what the host index no longer holds: an entry rafting_log_trim dropped, or one a moved index window
+// dropped (seglog_put), may still be named by the ring; the host then serves it, so both paths answer from the host index
+__device__ __forceinline__ bool step_probe(const ProbeD& d, uint32_t gid, int64_t index, const uint8_t*& rec, uint32_t& len) {
+    if (!seglog_hit(d.ring, d.K, d.arena, d.arena_bytes, d.oldest, gid, index, rec, len)) return false;
+    const Floor f = d.floor[gid];
+    return index >= f.index && *(const uint64_t*)(rec + 24) >= f.seq;            // SegHdr::seq
+}
+
+// t == P writes the identity, so that the scans' element P is the total
+__global__ void step_plan_count_kernel(StepPlansD s, GAgg* __restrict__ agg) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t > s.P) return;
+    const uint32_t c = t < s.P ? plan_entries(s.plan_meta[t]) : 0u;
+    agg[t] = GAgg{c, c ? 1u : 0u, 0};
+}
+
+// entries past refs_cap are neither probed nor written: the wait sizes them on the host
+__global__ void step_plan_probe_kernel(StepPlansD s, ProbeD d, const GAgg* __restrict__ off1, uint32_t refs_cap, GAgg* __restrict__ agg) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t > s.P) return;
+    GAgg v = {0, 0, 0};
+    const uint32_t c = t < s.P ? plan_entries(s.plan_meta[t]) : 0u;
+    if (c) {
+        const uint64_t first = off1[t].a;
+        const uint32_t gid = plan_gid(s, t);
+        const int64_t x = s.plan_pp[t].x;
+        for (uint32_t j = 0; j < c && first + j < refs_cap; j++) {
+            const uint8_t* rec; uint32_t len;
+            if (step_probe(d, gid, x + 1 + j, rec, len)) { v.a += ((uint64_t)len + 15) & ~15ull; v.c++; }
+            else v.b++;
+        }
     }
-    if (sub == 0) lens[en] = hit ? len : 0xffffffffu;
-    if (!hit) return;
-    const int4* src = (const int4*)(rec + sizeof(SegHdr));       // records and payloads are 16-byte aligned
-    int4* dst = (int4*)(out + q.out_off);                        // out_off is 16-byte aligned
-    const uint32_t words = (len + 15) >> 4;
-    for (uint32_t i = sub; i < words; i += 8) dst[i] = src[i];
+    agg[t] = v;
+}
+
+__global__ void step_plan_emit_kernel(StepPlansD s, ProbeD d, const GAgg* __restrict__ off1, const GAgg* __restrict__ off2, StepOutD o) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= s.P) return;
+    const uint32_t c = plan_entries(s.plan_meta[t]);
+    if (!c) return;
+    const GAgg p = off1[t];
+    GAgg q = off2[t];
+    if (p.b < o.plans_cap) { rafting_plan_ref_t r; r.slot = t; r.first = (uint32_t)p.a; r.count = c; r._pad = 0; o.plans[p.b] = r; }
+    const uint32_t gid = plan_gid(s, t);
+    const int64_t x = s.plan_pp[t].x;
+    for (uint32_t j = 0; j < c && p.a + j < o.refs_cap; j++) {
+        const uint64_t k = p.a + j;
+        rafting_entry_ref_t r; r.gid = gid; r.index = x + 1 + j;
+        const uint8_t* rec; uint32_t len;
+        if (step_probe(d, gid, r.index, rec, len)) {
+            r.len = len; r.term = *(const int64_t*)(rec + 16); r.blob_off = q.a;                 // SegHdr::term
+            GatherReq g; g.gid = gid; g.slot = (uint32_t)k; g.index = r.index; g.out_off = q.a;
+            q.a += ((uint64_t)len + 15) & ~15ull;
+            if (q.a > o.blob_cap) g.index = 0;        // past the blob: a request the ring never serves (indices start at 1)
+            o.req[q.c++] = g;
+        } else {
+            r.len = 0xffffffffu; r.term = 0; r.blob_off = 0;                                       // the wait fills them in
+            o.miss[q.b++] = (uint32_t)k;
+        }
+        o.refs[k] = r;
+    }
+}
+
+// total->c requests; a grid-stride loop, so the grid is sized without knowing their number
+__global__ void step_gather_copy_kernel(const GatherReq* __restrict__ req, const GAgg* __restrict__ total, const unsigned long long* __restrict__ ring,
+                                        uint32_t K, const uint8_t* __restrict__ arena, uint64_t arena_bytes, uint64_t oldest_resident,
+                                        uint32_t* __restrict__ lens, uint8_t* __restrict__ out) {
+    const uint64_t n = total->c;
+    for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; (t >> 3) < n; t += (uint64_t)gridDim.x * blockDim.x)
+        seglog_gather_entry(req[t >> 3], (uint32_t)(t & 7), ring, K, arena, arena_bytes, oldest_resident, lens + (t >> 3), out);
 }
 
 }  // namespace rafting
@@ -143,6 +264,7 @@ static void seglog_release(rafting_engine* e) {
     if (L->d_out) cudaFree(L->d_out);
     if (L->d_blob) cudaFree(L->d_blob);
     if (L->t0) { cudaEventDestroy(L->t0); cudaEventDestroy(L->t1); }
+    if (L->d_floor) cudaFree(L->d_floor);
     delete L; e->seglog = nullptr;
 }
 
@@ -156,10 +278,13 @@ extern "C" int rafting_log_config(rafting_engine_t* e, uint32_t segment_bytes, u
     L->seg_bytes = segment_bytes; L->nseg = hbm_segments; L->K = ring_slots;
     e->seglog = L;
     L->index.resize(e->G);
+    L->floor.assign(e->G, rafting::Floor{0, 0});
     const size_t ring = (size_t)e->G * ring_slots;
     CU(cudaMalloc(&L->arena, (size_t)segment_bytes * hbm_segments));
     CU(cudaMalloc(&L->ring, ring * 8));
     CU(cudaMemset(L->ring, 0, ring * 8));                          // 0 = empty slot
+    CU(cudaMalloc(&L->d_floor, (size_t)e->G * sizeof(rafting::Floor)));
+    CU(cudaMemset(L->d_floor, 0, (size_t)e->G * sizeof(rafting::Floor)));
     CU(cudaStreamCreateWithFlags(&L->s_spill, cudaStreamNonBlocking));
     CU(cudaStreamCreateWithFlags(&L->s_log, cudaStreamNonBlocking));
     CU(cudaEventCreateWithFlags(&L->ev_tables, cudaEventDisableTiming));
@@ -180,7 +305,24 @@ static inline void seglog_drop(SegLog* L, const HostLoc& h) {
     if (h.off != rafting::NO_ARENA) L->seg_live[h.off / L->seg_bytes]--;
     L->indexed--;
 }
-static inline void seglog_put(SegLog* L, uint32_t gid, int64_t index, const HostLoc& hl) {
+static inline void seglog_floor(SegLog* L, uint32_t gid, int64_t index, uint64_t seq) {
+    rafting::Floor& f = L->floor[gid];
+    if (index > f.index) f.index = index;
+    if (seq > f.seq) f.seq = seq;
+    if (gid < L->floor_lo) L->floor_lo = gid;
+    if (gid > L->floor_hi) L->floor_hi = gid;
+}
+// the changed floors go up on the log stream, ahead of every gather enqueued later (a pageable copy: the host may change them
+// again as soon as this returns)
+static int seglog_floor_flush(SegLog* L) {
+    if (L->floor_lo > L->floor_hi) return RAFTING_OK;
+    CU(cudaMemcpyAsync(L->d_floor + L->floor_lo, L->floor.data() + L->floor_lo, (size_t)(L->floor_hi - L->floor_lo + 1) * sizeof(rafting::Floor),
+                       cudaMemcpyHostToDevice, L->s_log));
+    L->floor_lo = UINT32_MAX; L->floor_hi = 0;
+    return RAFTING_OK;
+}
+// seq: the append sequence number the record gets (its SegHdr::seq)
+static inline void seglog_put(SegLog* L, uint32_t gid, int64_t index, const HostLoc& hl, uint64_t seq) {
     rafting::GroupIdx& gi = L->index[gid];
     const HostLoc none = {0, 0xffffffffu, 0, rafting::NO_FILE};
     if (gi.v.empty()) gi.base = index;
@@ -189,6 +331,7 @@ static inline void seglog_put(SegLog* L, uint32_t gid, int64_t index, const Host
     if (index < gi.base - SEGLOG_INDEX_WINDOW || index >= gi.base + (int64_t)gi.v.size() + SEGLOG_INDEX_WINDOW) {
         for (const HostLoc& h : gi.v) seglog_drop(L, h);
         gi.v.clear(); gi.base = index;
+        seglog_floor(L, gid, 0, seq);                              // every older record of the group is gone
     }
     if (index < gi.base) { gi.v.insert(gi.v.begin(), (size_t)(gi.base - index), none); gi.base = index; }
     if (index >= gi.base + (int64_t)gi.v.size()) gi.v.resize((size_t)(index - gi.base) + 1, none);
@@ -196,6 +339,7 @@ static inline void seglog_put(SegLog* L, uint32_t gid, int64_t index, const Host
         const size_t cut = gi.v.size() - (size_t)SEGLOG_INDEX_WINDOW;
         for (size_t k = 0; k < cut; k++) seglog_drop(L, gi.v[k]);
         gi.v.erase(gi.v.begin(), gi.v.begin() + (ptrdiff_t)cut); gi.base += (int64_t)cut;
+        seglog_floor(L, gid, gi.base, 0);
     }
     HostLoc& slot = gi.v[(size_t)(index - gi.base)];
     if (slot.len == 0xffffffffu) L->indexed++;
@@ -246,6 +390,7 @@ static int seglog_spill_for(rafting_engine* e, SegLog* L, uint64_t new_head) {
 static int seglog_wal_put(SegLog* L, const rafting_entry_ref_t* refs, uint32_t n, const uint8_t* blob, std::vector<uint64_t>& file_offs);
 static int log_append_impl(rafting_engine_t* e, const rafting_entry_ref_t* refs, uint32_t n, const void* blob, size_t blob_bytes) {
     if (!e || !e->seglog) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
+    if (e->seglog->step_gathers) return fail(RAFTING_E_BUSY, "a step gather has not been waited for (rafting_log_gather_step_wait)");
     if (n == 0) return RAFTING_OK;
     if (!refs || (!blob && blob_bytes)) return fail(RAFTING_E_INVAL, "null argument");
     SegLog* L = e->seglog;
@@ -294,7 +439,7 @@ static int log_append_impl(rafting_engine_t* e, const rafting_entry_ref_t* refs,
             r.gid = refs[i].gid; r.len = refs[i].len; r.index = refs[i].index; r.term = refs[i].term; r.loc = h2; r.src = refs[i].blob_off;
             HostLoc hl; hl.off = h2; hl.len = refs[i].len; hl.term = refs[i].term;
             hl.file_off = file_offs.empty() ? rafting::NO_FILE : file_offs[i];
-            seglog_put(L, refs[i].gid, refs[i].index, hl);
+            seglog_put(L, refs[i].gid, refs[i].index, hl, L->appended + m);
             head = h2 + rec; m++;
         }
         if (m == 0) return fail(RAFTING_E_CAPACITY, "arena too small for a single record");
@@ -312,7 +457,7 @@ static int log_append_impl(rafting_engine_t* e, const rafting_entry_ref_t* refs,
         CU(cudaGetLastError());
         L->head = head; L->appended += m; done += m;
     }
-    return RAFTING_OK;
+    return seglog_floor_flush(L);
 }
 
 // no C++ exception may cross the C ABI (a host index that cannot grow is RAFTING_E_NOMEM, not std::terminate)
@@ -340,6 +485,11 @@ static int seglog_range(rafting_engine* e, uint32_t gid, int64_t* lo, int64_t* h
     CU(cudaStreamSynchronize(L->s_log));
     if ((((uint32_t)meta >> rafting::W_NRUNS_SH) & 0xf) == 0) { *lo = 1; *hi = 0; }
     return RAFTING_OK;
+}
+// logical offset of the oldest byte the HBM arena still holds (the newest nseg segments)
+static inline uint64_t seglog_oldest_resident(const SegLog* L) {
+    const uint64_t newest = L->head ? (L->head - 1) / L->seg_bytes : 0;
+    return newest + 1 >= L->nseg ? (newest + 1 - L->nseg) * (uint64_t)L->seg_bytes : 0;
 }
 static inline bool seglog_resident(const SegLog* L, uint64_t off) {
     const uint64_t newest = L->head ? (L->head - 1) / L->seg_bytes : 0;
@@ -448,8 +598,7 @@ extern "C" int rafting_log_gather(rafting_engine_t* e, uint32_t n_ranges, const 
         uint32_t* d_lens = (uint32_t*)((uint8_t*)L->d_req + req_bytes);
         CU(cudaMemcpyAsync(L->d_req, req.data(), req_bytes, cudaMemcpyHostToDevice, L->s_log));
         if (!L->t0) { CU(cudaEventCreate(&L->t0)); CU(cudaEventCreate(&L->t1)); }
-        const uint64_t newest = L->head ? (L->head - 1) / L->seg_bytes : 0;
-        const uint64_t oldest = newest + 1 >= L->nseg ? (newest + 1 - L->nseg) * (uint64_t)L->seg_bytes : 0;
+        const uint64_t oldest = seglog_oldest_resident(L);
         CU(cudaEventRecord(L->t0, L->s_log));
         rafting::seglog_gather_kernel<<<(uint32_t)(((uint64_t)nq * 8 + 255) / 256), 256, 0, L->s_log>>>(
             (const GatherReq*)L->d_req, nq, L->ring, L->K, L->arena, (uint64_t)L->seg_bytes * L->nseg, oldest, d_lens, L->d_out);
@@ -479,12 +628,184 @@ extern "C" int rafting_log_gather(rafting_engine_t* e, uint32_t n_ranges, const 
     return RAFTING_OK;
 }
 
+// ---- rafting_log_gather_step_begin / _wait: the payloads of the plans of a slot's compact step ----
+// Per slot: device scratch of the passes, and a pinned (so mapped) block for the totals, the miss list and the outputs the
+// device cannot write directly
+struct StepGather {
+    Blk dev;                                   // off1 / off2 aggregates and scans, CUB's scratch, requests, the copy's lens
+    Blk host;                                  // totals (2 x GAgg), miss list [refs_cap], then the staged outputs
+    cudaEvent_t ev = nullptr, t0 = nullptr, t1 = nullptr;
+    bool timed = false;                        // the kernels ran (the step has plan columns)
+    rafting_entry_ref_t* refs = nullptr; uint32_t refs_cap = 0, plans_cap = 0; uint8_t* blob = nullptr; size_t blob_cap = 0;
+    rafting_plan_ref_t* plans = nullptr;
+    size_t o_miss = 0, o_refs = 0, o_plans = 0, o_blob = 0;   // offsets in host; the staged outputs only
+    bool st_refs = false, st_plans = false, st_blob = false;
+};
+static void step_gather_release(Slot& s) {
+    StepGather* g = s.gather;
+    if (!g) return;
+    if (g->ev) { cudaEventSynchronize(g->ev); cudaEventDestroy(g->ev); cudaEventDestroy(g->t0); cudaEventDestroy(g->t1); }
+    blk_free(g->dev, false); blk_free(g->host, true);
+    delete g; s.gather = nullptr;
+}
+// the device address of host memory the device can write (pinned or registered, aligned), else null
+static uint8_t* mapped_host(void* p, uintptr_t align) {
+    cudaPointerAttributes pa;
+    if (p && (uintptr_t)p % align == 0 && cudaPointerGetAttributes(&pa, p) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer)
+        return (uint8_t*)pa.devicePointer;
+    cudaGetLastError();
+    return nullptr;
+}
+
+extern "C" int rafting_log_gather_step_begin(rafting_engine_t* e, uint32_t slot, rafting_entry_ref_t* refs_out, uint32_t refs_cap,
+                                             void* blob_out, size_t blob_cap, rafting_plan_ref_t* plans_out, uint32_t plans_cap) {
+    using namespace rafting;
+    if (!e || slot >= RAFTING_HOST_SLOTS || (refs_cap && !refs_out) || (blob_cap && !blob_out) || (plans_cap && !plans_out))
+        return fail(RAFTING_E_INVAL, "bad argument");
+    if (!e->seglog) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
+    Slot* S = e->host ? &e->host->slot[slot] : nullptr;
+    if (S && S->gathering) return fail(RAFTING_E_BUSY, "slot %u holds a gather that has not been waited for", slot);
+    if (!S || !S->compact_step || S->inflight) return fail(RAFTING_E_INVAL, "slot %u: no finished compact step to gather for", slot);
+    const uint64_t P = S->dev_out.plan_meta ? (uint64_t)S->rows_ * S->n_ * e->F : 0;   // no op, no sweep row: no plan columns
+    if (P >= 0x7fffffffu) return fail(RAFTING_E_CAPACITY, "%llu lane slots: a step gather walks fewer than 2^31", (unsigned long long)P);
+    SegLog* L = e->seglog;
+    CU(cudaSetDevice(e->cfg.device));
+    if (!S->gather) S->gather = new StepGather();
+    StepGather& g = *S->gather;
+    if (!g.ev) {
+        CU(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
+        CU(cudaEventCreate(&g.t0)); CU(cudaEventCreate(&g.t1));
+    }
+    uint8_t* d_refs = mapped_host(refs_out, 8); uint8_t* d_plans = mapped_host(plans_out, 4); uint8_t* d_blob = mapped_host(blob_out, 16);
+    g.st_refs = refs_cap && !d_refs; g.st_plans = plans_cap && !d_plans; g.st_blob = blob_cap && !d_blob;
+    Carve hc;
+    hc.take(2 * sizeof(GAgg));
+    g.o_miss = hc.take((size_t)refs_cap * 4);
+    g.o_refs = g.st_refs ? hc.take((size_t)refs_cap * sizeof(rafting_entry_ref_t)) : 0;
+    g.o_plans = g.st_plans ? hc.take((size_t)plans_cap * sizeof(rafting_plan_ref_t)) : 0;
+    g.o_blob = g.st_blob ? hc.take(blob_cap) : 0;
+    size_t scan_tmp = 0;
+    if (P) CU(cub::DeviceScan::ExclusiveScan(nullptr, scan_tmp, (GAgg*)nullptr, (GAgg*)nullptr, GAggSum(), GAgg{0, 0, 0}, (int)(P + 1)));
+    Carve dc;
+    const size_t o_agg1 = dc.take((P + 1) * sizeof(GAgg)), o_off1 = dc.take((P + 1) * sizeof(GAgg));
+    const size_t o_agg2 = dc.take((P + 1) * sizeof(GAgg)), o_off2 = dc.take((P + 1) * sizeof(GAgg));
+    const size_t o_req = dc.take((size_t)refs_cap * sizeof(GatherReq)), o_lens = dc.take((size_t)refs_cap * 4), o_tmp = dc.take(scan_tmp);
+    int rc;
+    if ((rc = blk_reserve(g.host, hc.o, true)) || (P && (rc = blk_reserve(g.dev, dc.o, false)))) return rc;
+    uint8_t* hdev = nullptr;
+    CU(cudaHostGetDevicePointer((void**)&hdev, g.host.p, 0));
+    if (!d_refs && g.st_refs) d_refs = hdev + g.o_refs;
+    if (!d_plans && g.st_plans) d_plans = hdev + g.o_plans;
+    if (!d_blob && g.st_blob) d_blob = hdev + g.o_blob;
+    if ((rc = seglog_floor_flush(L))) return rc;
+    g.timed = P != 0;
+    if (P) {
+        GAgg* agg1 = (GAgg*)(g.dev.p + o_agg1); GAgg* off1 = (GAgg*)(g.dev.p + o_off1);
+        GAgg* agg2 = (GAgg*)(g.dev.p + o_agg2); GAgg* off2 = (GAgg*)(g.dev.p + o_off2);
+        StepPlansD sp; sp.plan_meta = S->dev_out.plan_meta; sp.plan_pp = S->dev_out.plan_pp; sp.gids = S->c_gids;
+        sp.n = (uint32_t)S->n_; sp.F = e->F; sp.P = (uint32_t)P;
+        ProbeD pd; pd.ring = L->ring; pd.K = L->K; pd.arena = L->arena; pd.arena_bytes = (uint64_t)L->seg_bytes * L->nseg;
+        pd.oldest = seglog_oldest_resident(L); pd.floor = L->d_floor;
+        StepOutD od; od.refs = (rafting_entry_ref_t*)d_refs; od.refs_cap = refs_cap; od.plans = (rafting_plan_ref_t*)d_plans;
+        od.plans_cap = plans_cap; od.blob_cap = blob_cap; od.req = (GatherReq*)(g.dev.p + o_req); od.miss = (uint32_t*)(hdev + g.o_miss);
+        const uint32_t blocks = (uint32_t)((P + 1 + 255) / 256);
+        CU(cudaEventRecord(g.t0, L->s_log));
+        step_plan_count_kernel<<<blocks, 256, 0, L->s_log>>>(sp, agg1);
+        size_t tb = scan_tmp;
+        CU(cub::DeviceScan::ExclusiveScan(g.dev.p + o_tmp, tb, agg1, off1, GAggSum(), GAgg{0, 0, 0}, (int)(P + 1), L->s_log));
+        step_plan_probe_kernel<<<blocks, 256, 0, L->s_log>>>(sp, pd, off1, refs_cap, agg2);
+        tb = scan_tmp;
+        CU(cub::DeviceScan::ExclusiveScan(g.dev.p + o_tmp, tb, agg2, off2, GAggSum(), GAgg{0, 0, 0}, (int)(P + 1), L->s_log));
+        step_plan_emit_kernel<<<blocks, 256, 0, L->s_log>>>(sp, pd, off1, off2, od);
+        const uint64_t copy_blocks = ((uint64_t)refs_cap * 8 + 255) / 256;
+        if (copy_blocks)
+            step_gather_copy_kernel<<<(uint32_t)(copy_blocks < 1056 ? copy_blocks : 1056), 256, 0, L->s_log>>>(
+                od.req, off2 + P, pd.ring, pd.K, pd.arena, pd.arena_bytes, pd.oldest, (uint32_t*)(g.dev.p + o_lens), d_blob);
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(g.t1, L->s_log));
+        CU(cudaMemcpyAsync(g.host.p, off1 + P, sizeof(GAgg), cudaMemcpyDeviceToHost, L->s_log));
+        CU(cudaMemcpyAsync(g.host.p + sizeof(GAgg), off2 + P, sizeof(GAgg), cudaMemcpyDeviceToHost, L->s_log));
+    } else {
+        memset(g.host.p, 0, 2 * sizeof(GAgg));
+    }
+    CU(cudaEventRecord(g.ev, L->s_log));
+    g.refs = refs_out; g.refs_cap = refs_cap; g.blob = (uint8_t*)blob_out; g.blob_cap = blob_cap; g.plans = plans_out; g.plans_cap = plans_cap;
+    S->gathering = true; L->step_gathers++;
+    return RAFTING_OK;
+}
+
+// Bytes the refs past refs_cap need (they were neither probed nor written): the plans decoded on the host, lengths from the
+// host index.  Only a wait that returns RAFTING_E_CAPACITY gets here.
+static int step_gather_overflow(rafting_engine* e, const Slot& S, uint32_t refs_cap, uint64_t* bytes) {
+    const size_t P = S.rows_ * S.n_ * e->F;
+    std::vector<uint64_t> meta(P); std::vector<rafting_i64x2_t> pp(P); std::vector<uint32_t> gids(S.c_gids ? S.n_ : 0);
+    CU(cudaMemcpy(meta.data(), S.dev_out.plan_meta, P * 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(pp.data(), S.dev_out.plan_pp, P * 16, cudaMemcpyDeviceToHost));
+    if (S.c_gids) CU(cudaMemcpy(gids.data(), S.c_gids, S.n_ * 4, cudaMemcpyDeviceToHost));
+    uint64_t k = 0;
+    for (size_t t = 0; t < P; t++) {
+        const uint32_t c = RAFTING_PLM_KIND(meta[t]) == RAFTING_PLAN_AE ? RAFTING_PLM_COUNT(meta[t]) : 0;
+        const size_t i = (t / e->F) % S.n_;
+        const uint32_t gid = S.c_gids ? gids[i] : (uint32_t)i;
+        for (uint32_t j = 0; j < c; j++, k++) {
+            if (k < refs_cap) continue;
+            const HostLoc* hl = seglog_find(e->seglog, gid, pp[t].x + 1 + j);
+            if (hl) *bytes += ((uint64_t)hl->len + 15) & ~15ull;
+        }
+    }
+    return RAFTING_OK;
+}
+
+extern "C" int rafting_log_gather_step_wait(rafting_engine_t* e, uint32_t slot, uint32_t* n_refs, size_t* bytes, uint32_t* n_plans,
+                                            uint32_t* host_served) {
+    using namespace rafting;
+    if (!e || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
+    Slot* S = e->host ? &e->host->slot[slot] : nullptr;
+    if (!S || !S->gathering) return fail(RAFTING_E_INVAL, "slot %u has no gather in flight", slot);
+    CU(cudaSetDevice(e->cfg.device));
+    SegLog* L = e->seglog; StepGather& g = *S->gather;
+    CU(cudaEventSynchronize(g.ev));
+    S->gathering = false; L->step_gathers--;
+    const GAgg t1 = ((const GAgg*)g.host.p)[0], t2 = ((const GAgg*)g.host.p)[1];   // (refs, plans), (device bytes, misses, hits)
+    if (g.st_refs) memcpy(g.refs, g.host.p + g.o_refs, (size_t)(t1.a < g.refs_cap ? t1.a : g.refs_cap) * sizeof(rafting_entry_ref_t));
+    if (g.st_plans) memcpy(g.plans, g.host.p + g.o_plans, (size_t)(t1.b < g.plans_cap ? t1.b : g.plans_cap) * sizeof(rafting_plan_ref_t));
+    if (g.st_blob) memcpy(g.blob, g.host.p + g.o_blob, (size_t)(t2.a < g.blob_cap ? t2.a : g.blob_cap));
+    // the misses: lengths and terms from the host index, payloads after the device's
+    const uint32_t* miss = (const uint32_t*)(g.host.p + g.o_miss);
+    uint64_t need = t2.a;
+    for (uint64_t m = 0; m < t2.b; m++) {
+        rafting_entry_ref_t& r = g.refs[miss[m]];
+        r.blob_off = need;
+        if (const HostLoc* hl = seglog_find(L, r.gid, r.index)) { r.len = hl->len; r.term = hl->term; need += ((uint64_t)hl->len + 15) & ~15ull; }
+    }
+    if (t1.a > g.refs_cap) { if (int rc = step_gather_overflow(e, *S, g.refs_cap, &need)) return rc; }
+    const bool fits = t1.a <= g.refs_cap && t1.b <= g.plans_cap && need <= g.blob_cap;
+    for (uint64_t m = 0; fits && m < t2.b; m++) {
+        const rafting_entry_ref_t& r = g.refs[miss[m]];
+        if (r.len == 0xffffffffu || r.len == 0) continue;
+        if (int rc = seglog_fetch(e, L, *seglog_find(L, r.gid, r.index), g.blob + r.blob_off)) return rc;
+    }
+    CU(cudaStreamSynchronize(L->s_log));
+    if (g.timed) CU(cudaEventElapsedTime(&L->last_gather_kernel_ms, g.t0, g.t1));
+    L->last_gather_bytes = need;
+    if (fits) L->hbm_hits += t2.c;
+    if (n_refs) *n_refs = (uint32_t)(t1.a < UINT32_MAX ? t1.a : UINT32_MAX);
+    if (bytes) *bytes = (size_t)need;
+    if (n_plans) *n_plans = (uint32_t)(t1.b < UINT32_MAX ? t1.b : UINT32_MAX);
+    if (host_served) *host_served = (uint32_t)t2.b;
+    if (!fits)
+        return fail(RAFTING_E_CAPACITY, "slot %u: the plans need %llu refs, %llu bytes and %llu plan records (caps %u, %zu, %u)", slot,
+                    (unsigned long long)t1.a, (unsigned long long)need, (unsigned long long)t1.b, g.refs_cap, g.blob_cap, g.plans_cap);
+    return RAFTING_OK;
+}
+
 // Garbage collection behind RaftLog.flush (RocksLog.java:228-242: deleteRange below the new epoch): index entries below
 // a group's lowest stored key are dropped, and a cold (pinned host) segment whose last live record went away is freed.
 // A segment with no live record is also never spilled in the first place (seglog_spill_for).
 extern "C" int rafting_log_trim(rafting_engine_t* e, uint32_t first_gid, uint32_t count, uint64_t* dropped_entries, uint64_t* freed_cold_bytes) {
     if (!e || !e->seglog) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
     if ((uint64_t)first_gid + count > e->G) return fail(RAFTING_E_CAPACITY, "gid range beyond max_groups");
+    if (e->seglog->step_gathers) return fail(RAFTING_E_BUSY, "a step gather has not been waited for (rafting_log_gather_step_wait)");
     SegLog* L = e->seglog;
     CU(cudaSetDevice(e->cfg.device));
     std::vector<uint64_t> meta(count); std::vector<int64_t> lo(count), hi(count);
@@ -513,7 +834,9 @@ extern "C" int rafting_log_trim(rafting_engine_t* e, uint32_t first_gid, uint32_
         }
         gi.v.erase(gi.v.begin(), gi.v.begin() + cut);
         gi.base += cut;
+        seglog_floor(L, first_gid + k, gi.base, 0);
     }
+    if (int rc = seglog_floor_flush(L)) return rc;
     for (size_t s = 0; s < L->cold.size(); s++) {
         if (!L->cold[s] || (s < L->seg_live.size() && L->seg_live[s] != 0)) continue;
         CU(cudaEventSynchronize(L->cold_ready[s]));
@@ -605,6 +928,7 @@ extern "C" int rafting_log_store_open(rafting_engine_t* e, const char* path, uin
     if (!e || !e->seglog || !path) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
     SegLog* L = e->seglog;
     if (L->wal_fd >= 0) return fail(RAFTING_E_INVAL, "entry file already open");
+    if (L->step_gathers) return fail(RAFTING_E_BUSY, "a step gather has not been waited for (rafting_log_gather_step_wait)");
     if (L->appended) return fail(RAFTING_E_INVAL, "open the entry file before the first append");
     try {
         const int fd = open(path, O_RDWR | O_CREAT, 0644);
@@ -623,7 +947,7 @@ extern "C" int rafting_log_store_open(rafting_engine_t* e, const char* path, uin
             if (h.kind == WAL_PUT) {
                 if (h.a <= 0) break;
                 HostLoc hl; hl.off = rafting::NO_ARENA; hl.len = h.len; hl.term = h.b; hl.file_off = pos + sizeof(h);
-                seglog_put(L, h.gid, h.a, hl);
+                seglog_put(L, h.gid, h.a, hl, 0);
             } else if (h.kind == WAL_RANGE) {
                 for (size_t k = 0; k < gi.v.size(); k++) {
                     const int64_t idx = gi.base + (int64_t)k;

@@ -40,6 +40,7 @@ EXPORTS = [
     "rafting_engine_counters", "rafting_abi_sizes", "rafting_checkpoint", "rafting_restore",
     "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_step_begin_compact_active", "rafting_step_begin_compact_sweep", "rafting_step_begin_compact_due", "rafting_timers_due_begin", "rafting_timers_due_wait", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
     "rafting_log_config", "rafting_log_append", "rafting_log_read", "rafting_log_gather", "rafting_log_trim", "rafting_log_stats",
+    "rafting_log_gather_step_begin", "rafting_log_gather_step_wait",
     "rafting_log_store_open", "rafting_log_sync", "rafting_log_mark", "rafting_log_recovered", "rafting_log_export_kv", "rafting_log_store_stats",
 ]
 
@@ -101,6 +102,10 @@ def lib():
         L.rafting_log_gather.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                          C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_size_t)]
         L.rafting_log_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+        L.rafting_log_gather_step_begin.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t,
+                                                    C.c_void_p, C.c_uint32]
+        L.rafting_log_gather_step_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_size_t),
+                                                   C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
         L.rafting_log_trim.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.rafting_log_store_open.argtypes = [C.c_void_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint64)]
         L.rafting_log_sync.argtypes = [C.c_void_p]
@@ -561,14 +566,66 @@ class Engine:
         n, nb = C.c_uint32(), C.c_size_t()
         _check(lib().rafting_log_gather(self._h, len(ranges), g.ctypes.data, f.ctypes.data, c.ctypes.data, refs.ctypes.data, cap,
                                         blob.ctypes.data, blob_cap, C.byref(n), C.byref(nb)), "rafting_log_gather")
+        return self._gathered(refs[:n.value], blob)
+
+    @staticmethod
+    def _gathered(refs, blob) -> list:
+        """refs (ENTRY_REF records) + blob -> [(gid, index, term, bytes | None)], as log_gather returns them"""
         out = []
-        for r in refs[:n.value]:
+        for r in refs:
             if int(r["len"]) == 0xFFFFFFFF:
                 out.append((int(r["gid"]), int(r["index"]), 0, None))
             else:
                 out.append((int(r["gid"]), int(r["index"]), int(r["term"]),
                             blob[int(r["blob_off"]):int(r["blob_off"]) + int(r["len"])].tobytes()))
         return out
+
+    def log_gather_step_begin(self, slot: int, refs: np.ndarray, blob: np.ndarray, plans: np.ndarray,
+                              refs_cap: int | None = None, blob_cap: int | None = None, plans_cap: int | None = None):
+        """rafting_log_gather_step_begin: gather, on the entry buffer's stream, the payloads of the AppendEntries plans of the
+        compact step last waited for in `slot`.  refs (ENTRY_REF), blob (uint8) and plans (abi.PLAN_REF) receive them; pinned
+        arrays are written by the device directly.  They must stay alive until log_gather_step_wait."""
+        for a, dt in ((refs, self.ENTRY_REF), (blob, np.dtype(np.uint8)), (plans, abi.PLAN_REF)):
+            if a.dtype != dt or not a.flags.c_contiguous:
+                raise TypeError(f"expected a contiguous {dt} array")
+        rc = len(refs) if refs_cap is None else refs_cap
+        bc = len(blob) if blob_cap is None else blob_cap
+        pc = len(plans) if plans_cap is None else plans_cap
+        if rc > len(refs) or bc > len(blob) or pc > len(plans):
+            raise ValueError("a cap beyond its buffer")
+        _check(lib().rafting_log_gather_step_begin(self._h, slot, refs.ctypes.data if len(refs) else None, rc,
+                                                   blob.ctypes.data if len(blob) else None, bc,
+                                                   plans.ctypes.data if len(plans) else None, pc), "rafting_log_gather_step_begin")
+
+    def log_gather_step_wait(self, slot: int) -> tuple[int, int, int, int]:
+        """-> (n_refs, bytes, n_plans, host_served).  A cap that was too small raises RaftingError (E_CAPACITY) whose `sizes`
+        holds the same tuple, with the sizes needed."""
+        n, b, p, h = C.c_uint32(), C.c_size_t(), C.c_uint32(), C.c_uint32()
+        rc = lib().rafting_log_gather_step_wait(self._h, slot, C.byref(n), C.byref(b), C.byref(p), C.byref(h))
+        sizes = (n.value, b.value, p.value, h.value)
+        if rc:
+            ex = RaftingError(rc, "rafting_log_gather_step_wait")
+            ex.sizes = sizes
+            raise ex
+        return sizes
+
+    def log_gather_step(self, slot: int = 0, refs_cap: int = 1 << 16, blob_cap: int = 1 << 24, plans_cap: int = 1 << 16):
+        """Synchronous: -> ([(gid, index, term, bytes | None)] as log_gather returns them, plan records (abi.PLAN_REF),
+        host_served).  Grows the buffers and gathers again when a cap was too small."""
+        while True:
+            refs = np.zeros(refs_cap, dtype=self.ENTRY_REF)
+            blob = np.zeros(blob_cap, dtype=np.uint8)
+            plans = np.zeros(plans_cap, dtype=abi.PLAN_REF)
+            self.log_gather_step_begin(slot, refs, blob, plans)
+            try:
+                n, _, p, h = self.log_gather_step_wait(slot)
+            except RaftingError as ex:
+                if ex.rc != -5:
+                    raise
+                n, b, p, _ = ex.sizes
+                refs_cap, blob_cap, plans_cap = max(refs_cap, n), max(blob_cap, b), max(plans_cap, p)
+                continue
+            return self._gathered(refs[:n], blob), plans[:p].copy(), h
 
     def log_stats(self) -> dict:
         v = np.zeros(11, dtype=np.uint64)

@@ -49,6 +49,9 @@ final class NativeEngine {
     static native int  logRead(long h, int gid, long first, int maxN, ByteBuffer refsOut, ByteBuffer blobOut, long blobCap);   // RaftLog.batch
     static native int  logGather(long h, int nRanges, ByteBuffer gids, ByteBuffer firsts, ByteBuffer counts,
                                  ByteBuffer refsOut, int refsCap, ByteBuffer blobOut, long blobCap);  // the AE plans of a step at once
+    static native void logGatherStepBegin(long h, int slot, ByteBuffer refsOut, int refsCap, ByteBuffer blobOut, long blobCap,
+                                          ByteBuffer plansOut, int plansCap);                     // rafting_log_gather_step_begin: a step's AE payloads
+    static native void logGatherStepWait(long h, int slot, long[] nRefsBytesNPlansHostServed);   // rafting_log_gather_step_wait
     static native void logTrim(long h, int first, int count);                                    // rafting_log_trim (behind RaftLog.flush)
     static native int  logRecovered(long h, int gid, ByteBuffer initOut, ByteBuffer runsOut, int cap);   // rafting_log_recovered
     static native void commInitAll(long[] engines);                                              // rafting_comm_init_all: ONE JVM, n shards

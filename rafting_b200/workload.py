@@ -83,6 +83,20 @@ def _listed(ib: abi.Inbox) -> abi.Inbox:
     return ib
 
 
+def _rows_of(prev_out: abi.Outbox | None, rows: int) -> abi.Outbox | None:
+    """prev_out as the generators read it: `rows` rows of row columns.  The C generators index the previous outbox with the
+    rows of the step they fill; an outbox with fewer rows (the one-row outbox of the election warm-up, before a multi-row
+    leader stream) is padded with rows that hold no plan, ballot or reply, so nothing past its columns is read."""
+    if prev_out is None or getattr(prev_out, "rows", rows) >= rows:
+        return prev_out
+    p = abi.Outbox(rows, prev_out.n, prev_out.F, prev_out.G)
+    for name, _, _ in abi.Outbox.ROW_COLS:
+        getattr(p, name)[:prev_out.rows] = getattr(prev_out, name)
+    for name, _ in abi.Outbox.GROUP_COLS:
+        getattr(p, name)[...] = getattr(prev_out, name)
+    return p
+
+
 def leader_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None, gids=None) -> abi.Inbox:
     """Host (numpy) inbox of one leader-steady-state step (over the active list gids when given, see _over)."""
     w, kw = _over(w, gids)
@@ -92,6 +106,7 @@ def leader_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None, gids=Non
     ic = ib.as_c()
     ic.op_cd = None
     ic.op_e = None
+    prev_out = _rows_of(prev_out, w.rows)
     leader_step(w, step, None if prev_out is None else prev_out.as_c(), ic)
     ib.op_cd = None
     ib.op_e = None
@@ -115,6 +130,7 @@ def vote_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None, gids=None)
     """config #3 (RequestVote storm, PreVote on): one host inbox (over the active list gids when given, see _over)."""
     w, kw = _over(w, gids)
     ib = _listed(abi.Inbox(w.rows, w.n, w.F, **kw))
+    prev_out = _rows_of(prev_out, w.rows)
     rc = _bind().rafting_wl_vote_step(C.byref(w), step, None if prev_out is None else C.byref(prev_out.as_c()),
                                       C.byref(ib.as_c()), 0, None)
     if rc:
@@ -129,6 +145,7 @@ def mixed_inbox_host(w: WlCfg, step: int, prev_out: abi.Outbox | None, gids=None
     ib = _listed(abi.Inbox(w.rows, w.n, w.F, ent_cap=POOL_TERMS, **kw))
     _bind().rafting_wl_fill_term_pool(ib.ent_terms.ctypes.data, POOL_TERMS, 0, None)
     ib.ent_count = POOL_TERMS
+    prev_out = _rows_of(prev_out, w.rows)
     rc = _bind().rafting_wl_mixed_step(C.byref(w), step, None if prev_out is None else C.byref(prev_out.as_c()),
                                        C.byref(ib.as_c()), 0, None)
     if rc:
