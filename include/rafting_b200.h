@@ -131,8 +131,19 @@ typedef struct rafting_cfg {
     int32_t  device;                /* CUDA ordinal                                            */
     uint32_t flags;                 /* RAFTING_CFG_* ; 0 = bit-identical to the reference      */
 } rafting_cfg_t;
-/* Opt-in departures from the reference that close the two flaws DESIGN.md §2 documents.  Specified and tested in the
-   oracle (tests/test_cluster_cpu.py); the CUDA engine of this version REJECTS a non-zero cfg.flags (RAFTING_E_INVAL). */
+/* Opt-in departures from the reference that close the two flaws DESIGN.md §2 documents.  The engine and the oracle honour
+   both bits on every step path; rafting_engine_create refuses any other bit (RAFTING_E_INVAL).
+   - flags == 0 is bit-identical to the reference, and its steps run exactly the kernels they ran before the bits existed.
+   - RAFTING_CFG_STRICT_CANDIDATE_VOTE: a Candidate that receives a RequestVote or PreVote of a higher term steps down at its
+     own term first, so the request is judged by Follower.requestVote with logUpToDate (Candidate.java:68-71 grants it
+     unchecked).  Election safety needs EVERY replica of a group to run with this bit: a cluster that mixes flagged and
+     unflagged replicas is as safe as the reference, no safer.
+   - RAFTING_CFG_LENIENT_FOLLOWER_COMMIT: an AppendEntries whose leaderCommit lies below the follower's commitIndex leaves
+     the commitIndex where it is instead of failing with RAFTING_ERR_COMMIT_ROLLBACK (Follower.java:76-82), so that a new
+     leader that knows a lower commitIndex no longer stalls its group.  RAFTING_ERR_COMMIT_ROLLBACK then never arises, and
+     the payload rule of INTEGRATION.md §4 reduces to "the reply says success".
+   The flags are engine configuration, not shard state: rafting_state_save does not record them, and a shard image saved
+   with one set of flags may be loaded into an engine created with another. */
 #define RAFTING_CFG_STRICT_CANDIDATE_VOTE   1u   /* a Candidate applies logUpToDate before it votes (Candidate.java:68-71 does not) */
 #define RAFTING_CFG_LENIENT_FOLLOWER_COMMIT 2u   /* leaderCommit below the follower's commitIndex is ignored instead of asserted */
 

@@ -82,14 +82,17 @@ FLAGS_LIB = os.path.join(HERE, "librafting_b200_flags.so")
 
 
 def build_flags(force: bool = False) -> str:
-    """The same engine compiled with -DRAFTING_ENABLE_CFG_FLAGS: the device branches of the two opt-in protocol fixes
-    (RAFTING_CFG_STRICT_CANDIDATE_VOTE, RAFTING_CFG_LENIENT_FOLLOWER_COMMIT).  A library of its own: the default build stays
-    byte-identical to the reference-faithful one and rejects a non-zero cfg.flags.  Loaded with RAFTING_B200_LIB=<path>."""
-    deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS] + [os.path.join(CSRC, h) for h in ("compact.cuh", "pair_kernel.cuh")]
-    cmd = [nvcc()] + NVCC_FLAGS + ["-DRAFTING_ENABLE_CFG_FLAGS"] + [os.path.join(CSRC, s) for s in SOURCES] + ["-o", FLAGS_LIB, "-ldl"]
-    if not force and up_to_date(FLAGS_LIB, deps, cmd):
-        return FLAGS_LIB
-    compile_lib(cmd, FLAGS_LIB, "nvcc (flags build)")
+    """The default library under a second name, for tests/test_cluster_gpu.py::test_opt_in_protocol_fixes_on_the_device_in_lock_step,
+    which loads it with RAFTING_B200_LIB=<path> and checks that the file name says "flags".  The opt-in protocol fixes
+    (RAFTING_CFG_STRICT_CANDIDATE_VOTE, RAFTING_CFG_LENIENT_FOLLOWER_COMMIT) are part of the default library, so this is the
+    same build of the same sources, copied rather than compiled twice; `force` forces the copy, not a second compile."""
+    lib = build()
+    if force or not up_to_date(FLAGS_LIB, [lib], [lib]):
+        if os.path.exists(FLAGS_LIB + ".cmd"):
+            os.remove(FLAGS_LIB + ".cmd")
+        shutil.copy(lib, FLAGS_LIB)
+        with open(FLAGS_LIB + ".cmd", "w") as f:
+            f.write(lib)
     return FLAGS_LIB
 
 

@@ -125,9 +125,8 @@ extern "C" const char* rafting_last_error(void) { return g_err; }
 extern "C" int rafting_engine_create(const rafting_cfg_t* cfg, rafting_engine_t** out) {
     if (!cfg || !out) return fail(RAFTING_E_INVAL, "null argument");
     if (cfg->struct_size != sizeof(rafting_cfg_t)) return fail(RAFTING_E_INVAL, "cfg.struct_size %u != %zu", cfg->struct_size, sizeof(rafting_cfg_t));
-#ifndef RAFTING_ENABLE_CFG_FLAGS
-    if (cfg->flags != 0) return fail(RAFTING_E_INVAL, "cfg.flags 0x%x: the opt-in protocol fixes exist in the oracle only in this version", cfg->flags);
-#endif
+    if (cfg->flags & ~(uint32_t)(RAFTING_CFG_STRICT_CANDIDATE_VOTE | RAFTING_CFG_LENIENT_FOLLOWER_COMMIT))
+        return fail(RAFTING_E_INVAL, "cfg.flags 0x%x: only RAFTING_CFG_STRICT_CANDIDATE_VOTE (1) and RAFTING_CFG_LENIENT_FOLLOWER_COMMIT (2) are defined", cfg->flags);
     if (cfg->replicas < 2 || cfg->replicas > RAFTING_MAX_REPLICAS || cfg->local_slot >= cfg->replicas || cfg->max_groups == 0)
         return fail(RAFTING_E_INVAL, "bad replicas/local_slot/max_groups");
     int ndev = 0;
@@ -143,9 +142,7 @@ extern "C" int rafting_engine_create(const rafting_cfg_t* cfg, rafting_engine_t*
     e->dcfg.pre_vote = cfg->pre_vote; e->dcfg.avail_critical_point = cfg->avail_critical_point;
     e->dcfg.recovery_cool_down_ms = cfg->recovery_cool_down_ms; e->dcfg.heartbeat_ms = cfg->heartbeat_ms;
     e->dcfg.election_ms = cfg->election_ms; e->dcfg.timer_seed = cfg->timer_seed;
-#ifdef RAFTING_ENABLE_CFG_FLAGS
     e->dcfg.flags = cfg->flags; e->dcfg._pad = 0;
-#endif
     int rc = 0;
     Tables& T = e->T; const size_t G = e->G, F = e->F;
     T.G = e->G; T.F = e->F;
@@ -301,17 +298,17 @@ extern "C" int rafting_group_close(rafting_engine_t* e, uint32_t gid) {
 // ---------------------------------------------------------------------------------------------
 // follower-slot bound FT and staging depth NST per replica count: R=2 -> <1,3>, R=3 -> <2,3>,
 // R<=5 -> <4,3>, R<=9 -> <8,2>, larger clusters keep their slots in local memory and read the inbox directly
-template <int FT, int NST>
+template <int FT, int NST, bool FIX>
 static int launch_t(rafting_engine* e, const InboxD& in, const OutboxD& out, cudaStream_t st) {
     const size_t smem = (size_t)NST * sizeof(Stage<FT>);
     static bool configured[64] = {false};
     if (smem > 0 && !configured[e->cfg.device & 63]) {
-        CU(cudaFuncSetAttribute(unrolled::step_kernel<FT, NST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CU(cudaFuncSetAttribute(unrolled::step_kernel<FT, NST, FIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured[e->cfg.device & 63] = true;
     }
     const uint32_t blocks = (in.n + TPB - 1) / TPB + (in.perm ? (uint32_t)NCLS : 0u);   // + NCLS: every class is padded to a block
     if (in.n == 0) return RAFTING_OK;
-    unrolled::step_kernel<FT, NST><<<blocks, TPB, smem, st>>>(e->T, in, out, e->d_cfg, e->dcfg);
+    unrolled::step_kernel<FT, NST, FIX><<<blocks, TPB, smem, st>>>(e->T, in, out, e->d_cfg, e->dcfg);
     return RAFTING_OK;
 }
 // R = 3, a step launched without a class sort (the leader stream): one thread per (group, follower) (pair_kernel.cuh, v7),
@@ -338,15 +335,18 @@ static int launch_pair(rafting_engine* e, const InboxD& in0, const OutboxD& out,
     CU(cudaLaunchKernelEx(&lc, pair::pair_kernel<NSTP>, e->T, in0, out, (const CfgD*)e->d_cfg, e->dcfg));
     return RAFTING_OK;
 }
+template <bool FIX>
 static int launch_looped(rafting_engine* e, const InboxD& in, const OutboxD& out, cudaStream_t st) {
     const uint32_t blocks = (in.n + TPB - 1) / TPB;
     if (blocks == 0) return RAFTING_OK;
-    looped::step_kernel<32, 0><<<blocks, TPB, 0, st>>>(e->T, in, out, e->d_cfg, e->dcfg);
+    looped::step_kernel<32, 0, FIX><<<blocks, TPB, 0, st>>>(e->T, in, out, e->d_cfg, e->dcfg);
     return RAFTING_OK;
 }
-static int launch_step(rafting_engine* e, const InboxD& in0, const OutboxD& out, cudaStream_t st) {
+// FIX: the kernels run with the opt-in protocol fixes compiled in (handlers.cuh).  Only the handlers of inbound requests
+// differ between the instantiations, so a step that carries none computes the same on both.
+template <bool FIX>
+static int launch_step_t(rafting_engine* e, const InboxD& in0, const OutboxD& out, cudaStream_t st) {
     int rc;
-    if ((uint64_t)in0.rows * in0.n * e->F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
     const uint32_t F = e->F;
     InboxD in = in0; in.perm = nullptr; in.perm_cnt = nullptr;
     // A step that may hold inbound requests mixes steady-state leaders with groups that need the generic handlers;
@@ -359,26 +359,35 @@ static int launch_step(rafting_engine* e, const InboxD& in0, const OutboxD& out,
     // at F = 2..4 the slow classes run in a kernel of their own, with their own register cap
     if (in.perm && F >= 2 && F <= 4) {
         const uint32_t sb = (in.n + unrolled::SLOW_TPB - 1) / unrolled::SLOW_TPB + (uint32_t)NCLS;
-        if (F == 2) unrolled::slow_kernel<2, 4><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
-        else unrolled::slow_kernel<4, 4><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
+        if (F == 2) unrolled::slow_kernel<2, 4, FIX><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
+        else unrolled::slow_kernel<4, 4, FIX><<<sb, unrolled::SLOW_TPB, 0, st>>>(e->T, in, out, e->d_cfg);
         in.flags |= INBOX_INTERNAL_SLOW_ELSEWHERE;
     }
-    if (F == 1) rc = launch_t<1, 3>(e, in, out, st);
+    if (F == 1) rc = launch_t<1, 3, FIX>(e, in, out, st);
 #ifndef RAFTING_NST2
 #define RAFTING_NST2 3
 #endif
     else if (F == 2) {
         // v7 (pair_kernel.cuh) measured faster than v6 on the leader stream on an H100 and slower on class-sorted steps
-        // (config #5), same-call A/Bs (DESIGN.md §5): it runs the steps launched without a class sort
-        rc = !in.perm ? launch_pair(e, in, out, st) : launch_t<2, RAFTING_NST2>(e, in, out, st);
+        // (config #5), same-call A/Bs (DESIGN.md §5): it runs the steps launched without a class sort.  pair_kernel has no
+        // FIX instantiation: with flags it takes only the steps that promise no inbound request, and the others run unsorted
+        // in the FIX step kernel
+        const bool pair = !in.perm && (!FIX || (in.flags & RAFTING_INBOX_NO_REQUESTS));
+        rc = pair ? launch_pair(e, in, out, st) : launch_t<2, RAFTING_NST2, FIX>(e, in, out, st);
     }
-    else if (F <= 4) rc = launch_t<4, 3>(e, in, out, st);
-    else if (F <= 8) rc = launch_t<8, 2>(e, in, out, st);
-    else rc = launch_looped(e, in, out, st);
+    else if (F <= 4) rc = launch_t<4, 3, FIX>(e, in, out, st);
+    else if (F <= 8) rc = launch_t<8, 2, FIX>(e, in, out, st);
+    else rc = launch_looped<FIX>(e, in, out, st);
     if (rc) return rc;
     e->launches++;
     CU(cudaGetLastError());
     return RAFTING_OK;
+}
+// Every step entry point (host, lease and leased steps, every compact begin, rafting_step_device and _seq) reaches the step
+// kernels here: the one place that picks the instantiation for the engine's cfg.flags
+static int launch_step(rafting_engine* e, const InboxD& in0, const OutboxD& out, cudaStream_t st) {
+    if ((uint64_t)in0.rows * in0.n * e->F >= (1ull << 32)) return fail(RAFTING_E_CAPACITY, "rows * groups * followers must stay below 2^32 per step");
+    return e->cfg.flags != 0 ? launch_step_t<true>(e, in0, out, st) : launch_step_t<false>(e, in0, out, st);
 }
 
 static void to_dev_views(const rafting_inbox_t* in, const rafting_outbox_t* out, uint32_t G, uint32_t* flags, InboxD& di, OutboxD& dout) {

@@ -274,7 +274,10 @@ __device__ __forceinline__ int log_up_to_date(const GS& g, int64_t index, int64_
     return index >= g.epochIndex;
 }
 
-// Follower.appendEntries body — Follower.java:52-87 + RocksLog.conflict/truncate/append (RocksLog.java:169-225)
+// Follower.appendEntries body — Follower.java:52-87 + RocksLog.conflict/truncate/append (RocksLog.java:169-225).
+// FIX: the instantiation of the kernels that honour cfg.flags (engine.cu launch_step); with FIX = false the opt-in branches
+// are not compiled, and the code is the reference's.
+template <bool FIX>
 __device__ __noinline__ int follower_append(GS& g, const Ctx& c, RowOut& ro, int peer, int64_t term, int64_t prevIndex,
                                             int64_t prevTerm, int64_t first, uint32_t n, const int64_t* terms,
                                             int64_t leaderCommit, Reply& rep) {
@@ -337,9 +340,8 @@ __device__ __noinline__ int follower_append(GS& g, const Ctx& c, RowOut& ro, int
         }
         if (!err && leaderCommit > g.epochIndex && nruns_of(g) > 0) {       // Follower.java:76-82
             int64_t ci = leaderCommit < g.hi ? leaderCommit : g.hi;
-#ifdef RAFTING_ENABLE_CFG_FLAGS
-            if ((c.cfg->flags & RAFTING_CFG_LENIENT_FOLLOWER_COMMIT) && ci < g.commit) ci = g.commit;   // ignored, not asserted
-#endif
+            if constexpr (FIX)
+                if ((c.cfg->flags & RAFTING_CFG_LENIENT_FOLLOWER_COMMIT) && ci < g.commit) ci = g.commit;   // ignored, not asserted
             err = commit_log(g, ci);
         }
     }
@@ -348,6 +350,7 @@ __device__ __noinline__ int follower_append(GS& g, const Ctx& c, RowOut& ro, int
     return err;
 }
 // Follower.appendEntries — Follower.java:35-88
+template <bool FIX>
 __device__ __forceinline__ int follower_append_entries(GS& g, const Ctx& c, RowOut& ro, int peer, int64_t term, int64_t prevIndex,
                                                        int64_t prevTerm, int64_t first, uint32_t n, const int64_t* terms,
                                                        int64_t leaderCommit, Reply& rep) {
@@ -360,8 +363,9 @@ __device__ __forceinline__ int follower_append_entries(GS& g, const Ctx& c, RowO
     } else if (leader_of(g) != -1 && peer != leader_of(g)) {
         return RAFTING_ERR_FOLLOWER_TWO_LEADERS;
     }
-    return follower_append(g, c, ro, peer, term, prevIndex, prevTerm, first, n, terms, leaderCommit, rep);
+    return follower_append<FIX>(g, c, ro, peer, term, prevIndex, prevTerm, first, n, terms, leaderCommit, rep);
 }
+template <bool FIX>
 __device__ __forceinline__ int op_append_entries(GS& g, const Ctx& c, RowOut& ro, int peer, int64_t term, int64_t prevIndex,
                                                  int64_t prevTerm, int64_t first, uint32_t n, const int64_t* terms,
                                                  int64_t leaderCommit, Reply& rep) {
@@ -377,7 +381,7 @@ __device__ __forceinline__ int op_append_entries(GS& g, const Ctx& c, RowOut& ro
         int err = switch_to(g, c, ro, RAFTING_ROLE_FOLLOWER, term, ballot_of(g));
         if (err) return err;
     }
-    return follower_append_entries(g, c, ro, peer, term, prevIndex, prevTerm, first, n, terms, leaderCommit, rep);
+    return follower_append_entries<FIX>(g, c, ro, peer, term, prevIndex, prevTerm, first, n, terms, leaderCommit, rep);
 }
 // Follower.requestVote — Follower.java:108-127
 __device__ __forceinline__ int follower_request_vote(GS& g, const Ctx& c, RowOut& ro, int peer, int64_t term, int64_t lastIndex,
@@ -392,6 +396,7 @@ __device__ __forceinline__ int follower_request_vote(GS& g, const Ctx& c, RowOut
     rep.valid = 1; rep.success = peer == ballot_of(g); rep.term = g.term;
     return 0;
 }
+template <bool FIX>
 __device__ __forceinline__ int op_request_vote(GS& g, const Ctx& c, RowOut& ro, int peer, int64_t term, int64_t lastIndex,
                                                int64_t lastTerm, Reply& rep) {
     const int role = role_of(g), self = (int)c.cfg->local_slot;
@@ -410,24 +415,26 @@ __device__ __forceinline__ int op_request_vote(GS& g, const Ctx& c, RowOut& ro, 
             if (peer != ballot_of(g)) { rep.valid = 1; rep.success = 0; rep.term = g.term; return 0; }
             else if (ballot_of(g) != self) return RAFTING_ERR_CANDIDATE_VOTE_SELF;
         }
-#ifdef RAFTING_ENABLE_CFG_FLAGS
-        // RAFTING_CFG_STRICT_CANDIDATE_VOTE: step down at the own term first (as Leader.java:106-108 does), so that
-        // Follower.requestVote applies logUpToDate to the higher-term request
-        const bool strict = (c.cfg->flags & RAFTING_CFG_STRICT_CANDIDATE_VOTE) && term > g.term;
-        int err = strict ? switch_to(g, c, ro, RAFTING_ROLE_FOLLOWER, g.term, ballot_of(g))
+        int err;
+        if constexpr (FIX) {
+            // RAFTING_CFG_STRICT_CANDIDATE_VOTE: step down at the own term first (as Leader.java:106-108 does), so that
+            // Follower.requestVote applies logUpToDate to the higher-term request
+            const bool strict = (c.cfg->flags & RAFTING_CFG_STRICT_CANDIDATE_VOTE) && term > g.term;
+            err = strict ? switch_to(g, c, ro, RAFTING_ROLE_FOLLOWER, g.term, ballot_of(g))
                          : switch_to(g, c, ro, RAFTING_ROLE_FOLLOWER, term, peer);
-#else
-        int err = switch_to(g, c, ro, RAFTING_ROLE_FOLLOWER, term, peer);
-#endif
+        } else {
+            err = switch_to(g, c, ro, RAFTING_ROLE_FOLLOWER, term, peer);
+        }
         if (err) return err;
     }
     return follower_request_vote(g, c, ro, peer, term, lastIndex, lastTerm, rep);
 }
+template <bool FIX>
 __device__ __forceinline__ int op_pre_vote(GS& g, const Ctx& c, RowOut& ro, int peer, int64_t term, int64_t lastIndex,
                                            int64_t lastTerm, Reply& rep) {
     const int role = role_of(g);
     if (role == RAFTING_ROLE_LEADER) { rep.valid = 1; rep.success = 0; rep.term = g.term; return 0; }   // Leader.java:88-91
-    if (role == RAFTING_ROLE_CANDIDATE) return op_request_vote(g, c, ro, peer, term, lastIndex, lastTerm, rep);  // Candidate.java:43-46
+    if (role == RAFTING_ROLE_CANDIDATE) return op_request_vote<FIX>(g, c, ro, peer, term, lastIndex, lastTerm, rep);  // Candidate.java:43-46
     if (term <= g.term || !(g.word & W_TIMEOUT_DET)) { rep.valid = 1; rep.success = 0; rep.term = g.term; return 0; }
     reset_timer(g, c, true, false);
     int up = log_up_to_date(g, lastIndex, lastTerm);

@@ -246,7 +246,7 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
             }
             __syncwarp(pmask);
             uint32_t dirty = g.dirty;
-            if (valid && f == 0) dirty = slow_row<2>(&ka, i, hg, r, kind, sweep, 1u | (hasEv ? 2u : 0u), 0u, g.dirty);
+            if (valid && f == 0) dirty = slow_row<2, false>(&ka, i, hg, r, kind, sweep, 1u | (hasEv ? 2u : 0u), 0u, g.dirty);
             if (f == 0) load_slab(T, hg, slab, tl);
             __syncwarp(pmask);
             dirty = __shfl_sync(pmask, dirty, lane & ~1u);
@@ -312,7 +312,7 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
                 if (valid) { store_lane(T, hl, x); if (f == 0) { g.inc = slab.inc[tl]; store_hot(T, hg, g); } }
                 __syncwarp(pmask);
                 uint32_t dirty = g.dirty;
-                if (valid && f == 0) dirty = slow_row<2>(&ka, i, hg, r, 0u, 0, 2u, bailAt, g.dirty);
+                if (valid && f == 0) dirty = slow_row<2, false>(&ka, i, hg, r, 0u, 0, 2u, bailAt, g.dirty);
                 if (f == 0) load_slab(T, hg, slab, tl);
                 __syncwarp(pmask);
                 dirty = __shfl_sync(pmask, dirty, lane & ~1u);

@@ -90,9 +90,7 @@ struct CfgD {
     int32_t  pre_vote, avail_critical_point;
     int64_t  recovery_cool_down_ms, heartbeat_ms, election_ms;
     uint64_t timer_seed;
-#ifdef RAFTING_ENABLE_CFG_FLAGS      // round-2 build switch (DESIGN.md §9-4): the opt-in protocol fixes on the device
-    uint32_t flags, _pad;
-#endif
+    uint32_t flags, _pad;           // rafting_cfg_t.flags: read only by the FIX instantiations of the step kernels
 };
 
 }  // namespace rafting

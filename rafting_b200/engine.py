@@ -24,7 +24,7 @@ import numpy as np
 from . import abi
 
 _LIB = None
-# RAFTING_B200_LIB selects another build of the same ABI (the -DRAFTING_ENABLE_CFG_FLAGS library, an A/B variant)
+# RAFTING_B200_LIB selects another build of the same ABI (a copy under another name, an A/B variant)
 _LIB_PATH = os.environ.get("RAFTING_B200_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "librafting_b200.so")
 
 STATUS = {0: "OK", -1: "E_INVAL", -2: "E_NOMEM", -3: "E_CUDA", -4: "E_CLOSED", -5: "E_CAPACITY",

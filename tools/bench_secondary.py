@@ -41,12 +41,12 @@ def init_array(G, **cols):
     return a
 
 
-def run(name, G, R, rows, steps, seed, gen, local_slot=0, elect=False, pool=False, quiet=False):
+def run(name, G, R, rows, steps, seed, gen, local_slot=0, elect=False, pool=False, quiet=False, flags=0, requests=True):
     import torch
     F = R - 1
     dev = torch.device("cuda:0")
     cfg = abi.make_cfg(replicas=R, local_slot=local_slot, max_groups=G, max_rows=rows, pre_vote=True,
-                       entry_pool_cap=workload.POOL_TERMS if pool else 0)
+                       entry_pool_cap=workload.POOL_TERMS if pool else 0, flags=flags)
     e = engine.Engine(cfg)
     if name == "config3":
         e.open_bulk(0, init_array(G, term=1 + np.arange(G) % 5, last_index=100 + np.arange(G) % 50,
@@ -55,7 +55,7 @@ def run(name, G, R, rows, steps, seed, gen, local_slot=0, elect=False, pool=Fals
         e.open_bulk(0, init_array(G, term=np.arange(G) % 7))
     st = torch.cuda.ExternalStream(e.stream(), device=dev)
     ob = [devbatch.DevOutbox(rows, G, F, G, dev) for _ in range(2)]
-    ib = devbatch.DevInbox(rows, G, F, dev, requests=True)
+    ib = devbatch.DevInbox(rows, G, F, dev, requests=requests)
     pool_t = None
     if pool:
         pool_t = torch.zeros(workload.POOL_TERMS, dtype=torch.int64, device=dev)
@@ -116,7 +116,7 @@ def run(name, G, R, rows, steps, seed, gen, local_slot=0, elect=False, pool=Fals
     alg = tot["acks"] * b_ack + (tot["votes"] + tot["vote_requests"]) * 64 + \
         (tot["ae_requests"] + tot["is_requests"]) * 160 + tot["entries"] * 32
     rec = {
-        "config": name, "groups": G, "replicas": R, "rows_per_step": rows, "steps": steps, "seed": hex(seed),
+        "config": name, "flags": flags, "groups": G, "replicas": R, "rows_per_step": rows, "steps": steps, "seed": hex(seed),
         "kernel_ms_total": sum(ms), "kernel_ms_per_step_median": float(np.median(ms)),
         "units": tot,
         "rates_per_s": {k: v / secs for k, v in tot.items() if v},
