@@ -454,8 +454,6 @@ extern "C" int rafting_step_begin_compact_req(rafting_engine_t* e, uint32_t slot
 
 // the device-chosen tail of a step begun with rafting_step_begin_compact_due (timers.cuh)
 struct DueTail { uint32_t n_host, cap; uint32_t* tail_out; };
-static int tail_reserve(rafting_engine* e, Blk& scratch);
-static int tail_select(rafting_engine* e, uint8_t* scratch, int64_t until, uint32_t* list, uint32_t n_host, uint32_t cap, uint32_t* n_due);
 
 // The list is checked in full before anything is enqueued: a lane's tag bitmap must have exactly one owning thread, and the
 // in-flight table is indexed by gid, so a duplicate or an id past max_groups would race on it or index past it.
@@ -478,6 +476,7 @@ struct CompactStep {
     bool list, has_reqs, has_sweep, el, pt;
     size_t n_req, n_oesc, ent_esc, pool;         // records, op escapes, entries the host sends, the step's entry pool
     Layout LD; CLayout LC; CRLayout LR;          // dense staging, wire blocks, request block
+    DueLayout LT;                                // a due step's tail selection (S.ctail)
     size_t w_counts, w_offs, w_tmp, scan_tmp;    // the request scan's scratch (S.creqw): order word, counts, offsets, CUB's
     size_t sweep_at;                             // offset of the sweep column in the staged copy of [gids | pad] sweep
     rafting_inbox_t din; rafting_outbox_t dout;  // the dense staging views the step kernel works on
@@ -558,7 +557,7 @@ static int compact_reserve(rafting_engine_t* e, Slot& S, CompactStep& p) {
     if ((rc = blk_reserve(S.din, p.LD.in_total, false)) || (rc = blk_reserve(S.dout, p.LD.out_total, false)) ||
         (rc = blk_reserve(S.cin, p.LC.in_total, false)) || (rc = blk_reserve(S.cout, p.LC.out_total, false)) ||
         (rc = blk_reserve(S.chout, 256 + (p.due ? (size_t)p.due->cap * 4 : 0), true))) return rc;
-    if (p.due && (rc = tail_reserve(e, S.ctail))) return rc;
+    if (p.due && ((rc = due_layout(e->G, p.LT)) || (rc = blk_reserve(S.ctail, p.LT.total, false)))) return rc;
     if (p.has_reqs && ((rc = blk_reserve(S.creq, p.LR.ent + p.pool * 8, false)) || (rc = blk_reserve(S.creqw, p.w_tmp + p.scan_tmp, false)))) return rc;
     rafting_inbox_t& d = p.din = stage_inbox(p.LD, S.din.p);
     if (!p.list) d.gids = nullptr;
@@ -629,7 +628,8 @@ static int compact_run(rafting_engine_t* e, Slot& S, const CompactStep& p) {
     if (p.due) {                                                               // the tail of the list, and counts[3]
         int64_t until = 0;
         for (size_t r = 0; r < rows; r++) until = p.sweep[r] > until ? p.sweep[r] : until;
-        if (int rc = tail_select(e, S.ctail.p, until, (uint32_t*)act.gids, p.due->n_host, p.due->cap, co.counts + 3)) return rc;
+        uint32_t* list = (uint32_t*)act.gids;
+        if (int rc = due_select(e, p.LT, S.ctail.p, until, list, p.due->n_host, list + p.due->n_host, p.due->cap, true, co.counts + 3, nullptr)) return rc;
     }
     InboxW dw;                                                                // unpack writes what the step kernel reads
     dw.op_meta = (uint64_t*)di.op_meta; dw.op_nr = (i64x2*)di.op_nr; dw.op_ab = (i64x2*)di.op_ab;

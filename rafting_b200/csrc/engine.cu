@@ -523,7 +523,7 @@ struct Slot {
     Blk creq, creqw;                          // compact path: request list + entry pool, and its scan scratch
     bool compact_step = false;                // the step in flight came through one of the rafting_step_begin_compact* calls
     rafting_coutbox_t c_host; uint32_t* c_counts_pinned = nullptr; void* c_esc_dev = nullptr;
-    Blk ctail;                                // rafting_step_begin_compact_due: the tail selection's scratch (timers.cuh)
+    Blk ctail;                                // rafting_step_begin_compact_due: the tail selection's scratch, due_layout (timers.cuh)
     uint32_t* c_tail_user = nullptr; uint32_t c_tail_n = 0;   // where the wait copies the tail (landed at chout + 256)
     Blk hin, hout;                            // pinned host staging (leases only), same layout as din / dout
     uint32_t* h_flags = nullptr;              // pinned landing place of the flag words on the caller-owned path
@@ -1276,6 +1276,6 @@ extern "C" int rafting_abi_sizes(uint32_t* out, uint32_t n) {
     return 7;
 }
 
-#include "compact.cuh"
 #include "timers.cuh"
+#include "compact.cuh"
 #include "seglog.cuh"

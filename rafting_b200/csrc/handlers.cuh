@@ -44,6 +44,17 @@ struct Reply { int valid, success; int64_t term; };
 
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ int role_of(const GS& g) { return (int)(g.word & W_ROLE_MASK); }
+// The sweep's firing rule on a group's meta word and timer: a sweep row at time t fires the implied TIMEOUT of a live group whose
+// timer is at or before t, where a follower's or candidate's timer of 0 or INT64_MAX never fires.  The step kernels and the due
+// selection (timers.cuh) must agree on it exactly, so this is its only statement.  The timer is taken by reference so that a
+// caller whose GS lives in local memory (slow_group) reads it only once the tests before it have passed.
+__device__ __forceinline__ bool timer_fires(uint32_t word, const int64_t& timer, int64_t t) {
+    if (!(word & W_ALIVE)) return false;
+    if ((word & W_ROLE_MASK) == RAFTING_ROLE_LEADER) return timer <= t;
+    return timer > 0 && timer != I64MAX && timer <= t;
+}
+// armed: some sweep, however late, fires it
+__device__ __forceinline__ bool timer_armed(uint32_t word, int64_t timer) { return timer_fires(word, timer, I64MAX); }
 __device__ __forceinline__ int ballot_of(const GS& g) { return (int)((g.word >> W_BALLOT_SH) & 0xff) - 1; }
 __device__ __forceinline__ int leader_of(const GS& g) { return (int)((g.word >> W_LEADER_SH) & 0xff) - 1; }
 __device__ __forceinline__ int nruns_of(const GS& g) { return (int)((g.word >> W_NRUNS_SH) & 0xf); }

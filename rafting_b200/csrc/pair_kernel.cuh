@@ -183,9 +183,7 @@ pair_kernel(Tables T, InboxD in, OutboxD out, const CfgD* __restrict__ cfgp, Cfg
         uint32_t repMeta = 0;
         uint64_t pm = 0; int64_t p0 = 0, p1 = 0, l0 = 0, l1 = 0;       // this lane's plan
         if (sweep != 0) {
-            const bool due = alive && ((role_of(g) == RAFTING_ROLE_LEADER) ? (g.timer <= sweep)
-                                       : (g.timer > 0 && g.timer != I64MAX && g.timer <= sweep));
-            if (due) { kind = RAFTING_OP_TIMEOUT; slowOp = true; }
+            if (timer_fires(g.word, g.timer, sweep)) { kind = RAFTING_OP_TIMEOUT; slowOp = true; }
         } else if (hasOps) {
             meta = (uint32_t)st.op_meta[tl]; now = st.op_nr[tl].x;
             const bool unav = hasAb && (((uint64_t)st.op_ab[tl].x >> f) & 1ull) != 0;

@@ -1,24 +1,32 @@
-// timers.cuh — the list of groups whose timers are due (include/rafting_b200.h, rafting_timers_due_begin).
+// timers.cuh — the groups whose timers are due: the due query (include/rafting_b200.h, rafting_timers_due_begin) and the tail
+// of a due step (rafting_step_begin_compact_due, compact.cuh).
 //
 // A sweep row at time t (rafting_inbox_t.row_now[r] = t) fires the implied RAFTING_OP_TIMEOUT of every listed group for which
-//     alive && (leader ? timer <= t : timer > 0 && timer != INT64_MAX && timer <= t)
-// holds (step_body.inc, pair_kernel.cuh).  A pump that runs steps over active lists needs to know, without holding the timers
-// on the host, which groups a sweep at t would fire.  Three launches on the engine's step stream (so a query sees every step
-// begun before it) answer that from g_meta and g_timer:
+// timer_fires (handlers.cuh) holds.  A pump that runs steps over active lists needs to know, without holding the timers on the
+// host, which groups a sweep at t would fire.  due_select answers that from g_meta and g_timer with launches on the engine's
+// step stream (so it sees every step begun before it):
 //
-//   due_scan_kernel   one thread per group reads its two 8-byte words (16 B per group): the due bit goes into a 32-bit warp
-//                     mask, and each block leaves (number due, earliest armed deadline after t) for the scan
-//   cub::DeviceScan   exclusive scan of the block pairs (sum, min): every block's first output position, and from the last
-//                     block the count and next deadline of the whole shard
-//   due_emit_kernel   one thread per group again, from the masks only (1 bit per group): the due gids, in increasing order,
-//                     at their positions below cap; the last block writes (count, next deadline)
+//   due_member_kernel  only when a host list is given: one thread per listed gid sets its bit in a G-bit mask (zeroed before)
+//   due_scan_kernel    one thread per group reads its two 8-byte words (16 B per group): an unlisted group is due or idle, each
+//                      bit goes into a 32-bit warp mask (the idle one only with fillers), and each block leaves a DueAgg (number due, number idle, earliest armed
+//                      deadline after t)
+//   cub::DeviceScan    exclusive scan of the block aggregates (sum, sum, min): every block's first due and first idle position
+//   due_emit_kernel    one thread per group again, from the masks only: the due gids in increasing order at [0, cap), then,
+//                      when asked for, the idle ones (fillers) from min(due total, cap); the last block writes the due total and
+//                      the next deadline
 //
 // The order-preserving compaction is a two-pass block scan instead of CUB DeviceSelect: DeviceSelect cannot stop at cap
 // entries (it writes every selected item), and the min-reduction of the deadlines would be a second pass over the 16 B per
-// group; here the scan carries the count and the minimum together, and the second pass reads 4 B per 32 groups.
-// The list is written where the caller reads it: into the caller's buffer directly when it is mapped pinned memory (every
-// cudaHostAlloc / pinned allocation on a 64-bit host), else into a mapped pinned staging block of the query slot, copied into the
-// caller's buffer at the wait.  Either way only the n_due entries cross PCIe, not cap; DESIGN.md "Timers" has the measurement.
+// group; here the scan carries the counts and the minimum together, and the second pass reads 4 B per 32 groups (8 B with
+// fillers).  Fillers are a template parameter of the scan and emit kernels, so the query, which never asks for them, neither
+// ballots nor stores nor reads the idle mask.
+//
+// The query lists nothing and asks for no fillers.  Its list is written where the caller reads it: into the caller's buffer
+// directly when it is mapped pinned memory (every cudaHostAlloc / pinned allocation on a 64-bit host), else into a mapped pinned
+// staging block of the query slot, copied into the caller's buffer at the wait.  Either way only the n_due entries cross PCIe,
+// not cap; DESIGN.md "Timers" has the measurement.
+// A due step lists the host's gids and asks for fillers: they keep the step's n host-known, so unpack / step / pack run unchanged
+// over the device-written gids column, and a listed group with no event whose timer is not due is left untouched by a sweep row.
 //
 // Included at the end of engine.cu (same translation unit: it uses rafting_engine, HostPath, fail(), CU()).
 #pragma once
@@ -26,182 +34,139 @@
 
 namespace rafting {
 
-constexpr uint32_t DUE_TPB = 256;
+constexpr uint32_t DUE_TPB = 256, DUE_WARPS = DUE_TPB / 32;
 
-struct DueAgg { uint32_t count, _pad; int64_t next; };      // due groups of a block, earliest armed deadline after `until`
+// unlisted groups due at `until`, unlisted groups not due, earliest armed deadline after `until` (of a block, then of a prefix)
+struct DueAgg { uint32_t due, idle; int64_t next; };
 struct DueAggOp {
     __host__ __device__ DueAgg operator()(const DueAgg& a, const DueAgg& b) const {
-        DueAgg r; r.count = a.count + b.count; r._pad = 0; r.next = a.next < b.next ? a.next : b.next; return r;
+        return DueAgg{a.due + b.due, a.idle + b.idle, a.next < b.next ? a.next : b.next};
     }
 };
-struct DueResult { uint32_t n_due, _pad; int64_t next; };   // what the wait reports, written by the last block of due_emit_kernel
+struct DueResult { uint32_t n_due, _pad; int64_t next; };   // what the query's wait reports, written by due_emit_kernel
 
-__global__ void __launch_bounds__(DUE_TPB) due_scan_kernel(Tables T, int64_t until, uint32_t* __restrict__ mask, DueAgg* __restrict__ agg) {
-    __shared__ uint32_t wcnt[DUE_TPB / 32];
-    __shared__ int64_t wmin[DUE_TPB / 32];
-    const uint32_t g = blockIdx.x * DUE_TPB + threadIdx.x;
-    bool due = false; int64_t next = I64MAX;
-    if (g < T.G) {
-        const uint32_t w = (uint32_t)T.g_meta[g];
-        const int64_t timer = T.g_timer[g];
-        const bool alive = (w & W_ALIVE) != 0, leader = (w & W_ROLE_MASK) == RAFTING_ROLE_LEADER;
-        // the sweep's predicate at t = until; a deadline it would fire at a later t is armed
-        const bool armed = alive && (leader || (timer > 0 && timer != I64MAX));
-        due = armed && timer <= until;
-        if (armed && timer > until) next = timer;
-    }
-    const uint32_t lane = threadIdx.x & 31u, wq = threadIdx.x >> 5;
-    const uint32_t m = __ballot_sync(0xffffffffu, due);
-    for (int o = 16; o > 0; o >>= 1) { const int64_t v = __shfl_down_sync(0xffffffffu, next, o); next = v < next ? v : next; }
-    if (lane == 0) { mask[(size_t)blockIdx.x * (DUE_TPB / 32) + wq] = m; wcnt[wq] = __popc(m); wmin[wq] = next; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        DueAgg a; a.count = 0; a._pad = 0; a.next = I64MAX;
-        for (uint32_t k = 0; k < DUE_TPB / 32; k++) { a.count += wcnt[k]; if (wmin[k] < a.next) a.next = wmin[k]; }
-        agg[blockIdx.x] = a;
-    }
-}
-
-__global__ void __launch_bounds__(DUE_TPB) due_emit_kernel(const uint32_t* __restrict__ mask, const DueAgg* __restrict__ agg,
-                                                           const DueAgg* __restrict__ off, uint32_t nblocks, uint32_t* __restrict__ out,
-                                                           uint32_t cap, DueResult* __restrict__ res) {
-    __shared__ uint32_t wbase[DUE_TPB / 32];
-    const uint32_t lane = threadIdx.x & 31u, wq = threadIdx.x >> 5;
-    const uint32_t* bm = mask + (size_t)blockIdx.x * (DUE_TPB / 32);
-    if (threadIdx.x == 0) {
-        uint32_t b = off[blockIdx.x].count;
-        for (uint32_t k = 0; k < DUE_TPB / 32; k++) { wbase[k] = b; b += __popc(bm[k]); }
-    }
-    __syncthreads();
-    const uint32_t m = bm[wq];
-    if ((m >> lane) & 1u) {
-        const uint32_t pos = wbase[wq] + __popc(m & ((1u << lane) - 1u));
-        if (pos < cap) out[pos] = blockIdx.x * DUE_TPB + threadIdx.x;
-    }
-    if (blockIdx.x == nblocks - 1 && threadIdx.x == 0) {
-        const DueAgg t = DueAggOp()(off[blockIdx.x], agg[blockIdx.x]);
-        DueResult r; r.n_due = t.count; r._pad = 0; r.next = t.next;
-        *res = r;
-    }
-}
-
-// ---- the tail of a step begun with rafting_step_begin_compact_due ----
-// The step's list is the host's gids (positions 0 .. n_host) followed by a tail of cap gids chosen on the step stream, after
-// the slot's H2D copy and before unpack_kernel, so the choice sees the state the step itself will see:
-//   tail_member_kernel   one thread per host position sets its gid's bit in a G-bit mask (zeroed by a memset before it)
-//   tail_scan_kernel     one thread per group, due_scan_kernel's predicate: a due-unlisted and an idle-unlisted bit go into two
-//                        warp masks, and each block leaves its two counts packed in one word, due << 32 | idle, so that one
-//                        cub::DeviceScan sum carries both (each count stays below 2^32: no carry crosses)
-//   tail_emit_kernel     due gids from tail position 0, then idle ones (fillers) from min(due total, cap), both in increasing
-//                        order, stopping at cap; one thread writes the due total (counts[3])
-// Fillers keep the step's n host-known, so unpack / step / pack run unchanged over the device-written gids column: a listed
-// group with no event whose timer is not due is left untouched by a sweep row.  DueAgg does not fit here (two counts, no
-// deadline), hence the packed sum.
-constexpr uint32_t TAIL_WARPS = DUE_TPB / 32;
-
-__global__ void tail_member_kernel(const uint32_t* __restrict__ gids, uint32_t n_host, uint32_t* __restrict__ member) {
+__global__ void due_member_kernel(const uint32_t* __restrict__ gids, uint32_t n_host, uint32_t* __restrict__ member) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k < n_host) { const uint32_t g = gids[k]; atomicOr(member + (g >> 5), 1u << (g & 31u)); }
 }
 
-__global__ void __launch_bounds__(DUE_TPB) tail_scan_kernel(Tables T, int64_t until, const uint32_t* __restrict__ member,
-                                                            uint32_t* __restrict__ mask, uint64_t* __restrict__ agg) {
-    __shared__ uint32_t wdue[TAIL_WARPS], widle[TAIL_WARPS];
+// member: the G-bit mask of the listed groups, or null when nothing is listed.  FILL: the idle groups are counted and get a
+// second warp mask (mask holds 2 words per warp, else 1); without it a block's idle count is 0.
+template <bool FILL>
+__global__ void __launch_bounds__(DUE_TPB) due_scan_kernel(Tables T, int64_t until, const uint32_t* __restrict__ member,
+                                                           uint32_t* __restrict__ mask, DueAgg* __restrict__ agg) {
+    __shared__ uint32_t wdue[DUE_WARPS], widle[DUE_WARPS];
+    __shared__ int64_t wmin[DUE_WARPS];
     const uint32_t g = blockIdx.x * DUE_TPB + threadIdx.x;
-    bool due = false, idle = false;
+    bool due = false, idle = false; int64_t next = I64MAX;
     if (g < T.G) {
         const uint32_t w = (uint32_t)T.g_meta[g];
         const int64_t timer = T.g_timer[g];
-        const bool alive = (w & W_ALIVE) != 0, leader = (w & W_ROLE_MASK) == RAFTING_ROLE_LEADER;
-        const bool armed = alive && (leader || (timer > 0 && timer != I64MAX));
-        const bool listed = (member[g >> 5] >> (g & 31u)) & 1u;
-        due = !listed && armed && timer <= until;
+        const bool listed = member && ((member[g >> 5] >> (g & 31u)) & 1u);
+        due = !listed && timer_fires(w, timer, until);
         idle = !listed && !due;
+        if (timer_armed(w, timer) && timer > until) next = timer;            // a later sweep would fire it
     }
     const uint32_t lane = threadIdx.x & 31u, wq = threadIdx.x >> 5;
-    const uint32_t md = __ballot_sync(0xffffffffu, due), mi = __ballot_sync(0xffffffffu, idle);
+    const uint32_t md = __ballot_sync(0xffffffffu, due), mi = FILL ? __ballot_sync(0xffffffffu, idle) : 0u;
+    for (int o = 16; o > 0; o >>= 1) { const int64_t v = __shfl_down_sync(0xffffffffu, next, o); next = v < next ? v : next; }
     if (lane == 0) {
-        const size_t at = ((size_t)blockIdx.x * TAIL_WARPS + wq) * 2;
-        mask[at] = md; mask[at + 1] = mi; wdue[wq] = __popc(md); widle[wq] = __popc(mi);
+        const size_t at = (size_t)blockIdx.x * DUE_WARPS + wq;
+        if (FILL) { mask[2 * at] = md; mask[2 * at + 1] = mi; } else mask[at] = md;
+        wdue[wq] = __popc(md); widle[wq] = __popc(mi); wmin[wq] = next;
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        uint64_t d = 0, i = 0;
-        for (uint32_t k = 0; k < TAIL_WARPS; k++) { d += wdue[k]; i += widle[k]; }
-        agg[blockIdx.x] = (d << 32) | i;
+        DueAgg a{0, 0, I64MAX};
+        for (uint32_t k = 0; k < DUE_WARPS; k++) a = DueAggOp()(a, DueAgg{wdue[k], widle[k], wmin[k]});
+        agg[blockIdx.x] = a;
     }
 }
 
-__global__ void __launch_bounds__(DUE_TPB) tail_emit_kernel(const uint32_t* __restrict__ mask, const uint64_t* __restrict__ agg,
-                                                            const uint64_t* __restrict__ off, uint32_t nblocks,
-                                                            uint32_t* __restrict__ tail, uint32_t cap, uint32_t* __restrict__ n_due) {
-    __shared__ uint32_t bdue[TAIL_WARPS], bidle[TAIL_WARPS];
-    const uint64_t total = off[nblocks - 1] + agg[nblocks - 1];
-    const uint32_t due_total = (uint32_t)(total >> 32), first_filler = due_total < cap ? due_total : cap;
-    if (blockIdx.x == 0 && threadIdx.x == 0) *n_due = due_total;
-    const uint64_t o = off[blockIdx.x];
-    const uint32_t od = (uint32_t)(o >> 32), oi = (uint32_t)o;
-    if (od >= cap && (uint64_t)first_filler + oi >= cap) return;          // every entry of this block lies past the tail
-    const uint32_t* bm = mask + (size_t)blockIdx.x * TAIL_WARPS * 2;
+// out[0, cap): the due gids, then (FILL) the idle ones, each in increasing order; the last block writes *n_due and, unless next
+// is null, *next.  A block whose positions all lie past cap returns once the totals are out.
+template <bool FILL>
+__global__ void __launch_bounds__(DUE_TPB) due_emit_kernel(const uint32_t* __restrict__ mask, const DueAgg* __restrict__ agg,
+                                                           const DueAgg* __restrict__ off, uint32_t nblocks, uint32_t* __restrict__ out,
+                                                           uint32_t cap, uint32_t* __restrict__ n_due, int64_t* __restrict__ next) {
+    constexpr uint32_t MW = FILL ? 2 : 1;                                  // mask words per warp
+    __shared__ uint32_t bdue[DUE_WARPS], bidle[DUE_WARPS];
+    if (blockIdx.x == nblocks - 1 && threadIdx.x == 0) {
+        const DueAgg t = DueAggOp()(off[blockIdx.x], agg[blockIdx.x]);
+        *n_due = t.due;
+        if (next) *next = t.next;
+    }
+    uint32_t first_filler = 0;
+    if (FILL) { const uint32_t d = off[nblocks - 1].due + agg[nblocks - 1].due; first_filler = d < cap ? d : cap; }
+    const DueAgg o = off[blockIdx.x];
+    if (o.due >= cap && (!FILL || (uint64_t)first_filler + o.idle >= cap)) return;
+    const uint32_t* bm = mask + (size_t)blockIdx.x * DUE_WARPS * MW;
     if (threadIdx.x == 0) {
-        uint32_t d = od, i = oi;
-        for (uint32_t k = 0; k < TAIL_WARPS; k++) { bdue[k] = d; bidle[k] = i; d += __popc(bm[2 * k]); i += __popc(bm[2 * k + 1]); }
+        uint32_t d = o.due, i = o.idle;
+        for (uint32_t k = 0; k < DUE_WARPS; k++) {
+            bdue[k] = d; d += __popc(bm[MW * k]);
+            if (FILL) { bidle[k] = i; i += __popc(bm[MW * k + 1]); }
+        }
     }
     __syncthreads();
     const uint32_t lane = threadIdx.x & 31u, wq = threadIdx.x >> 5, below = (1u << lane) - 1u;
-    const uint32_t md = bm[2 * wq], mi = bm[2 * wq + 1];
+    const uint32_t md = bm[MW * wq];
     const uint32_t g = blockIdx.x * DUE_TPB + threadIdx.x;
     if ((md >> lane) & 1u) {
         const uint32_t pos = bdue[wq] + __popc(md & below);
-        if (pos < cap) tail[pos] = g;
-    } else if ((mi >> lane) & 1u) {
-        const uint64_t pos = (uint64_t)first_filler + bidle[wq] + __popc(mi & below);
-        if (pos < cap) tail[pos] = g;
+        if (pos < cap) out[pos] = g;
+    } else if (FILL) {
+        const uint32_t mi = bm[MW * wq + 1];
+        if ((mi >> lane) & 1u) {
+            const uint64_t pos = (uint64_t)first_filler + bidle[wq] + __popc(mi & below);
+            if (pos < cap) out[pos] = g;
+        }
     }
 }
 
 }  // namespace rafting
 
-// device scratch of one tail selection over G groups: member mask, warp masks, block counts, their scan, CUB's scratch
-struct TailLayout { size_t member, mask, agg, off, tmp, total; uint32_t nblocks; };
-static int tail_layout(uint32_t G, TailLayout& L) {
+// device scratch of one selection over G groups: member mask, warp masks, block aggregates, their scan, CUB's scratch
+struct DueLayout { size_t member, mask, agg, off, tmp, total; uint32_t nblocks; };
+static int due_layout(uint32_t G, DueLayout& L) {
     using namespace rafting;
     L.nblocks = (G + DUE_TPB - 1) / DUE_TPB;
     size_t scan_tmp = 0;
-    CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)L.nblocks));
+    CU(cub::DeviceScan::ExclusiveScan(nullptr, scan_tmp, (DueAgg*)nullptr, (DueAgg*)nullptr, DueAggOp(), DueAgg{0, 0, I64MAX}, (int)L.nblocks));
     Carve c;
-    L.member = c.take((size_t)L.nblocks * TAIL_WARPS * 4); L.mask = c.take((size_t)L.nblocks * TAIL_WARPS * 8);
-    L.agg = c.take((size_t)L.nblocks * 8); L.off = c.take((size_t)L.nblocks * 8); L.tmp = c.take(scan_tmp);
+    L.member = c.take((size_t)L.nblocks * DUE_WARPS * 4); L.mask = c.take((size_t)L.nblocks * DUE_WARPS * 8);
+    L.agg = c.take((size_t)L.nblocks * sizeof(DueAgg)); L.off = c.take((size_t)L.nblocks * sizeof(DueAgg)); L.tmp = c.take(scan_tmp);
     L.total = c.o;
     return RAFTING_OK;
 }
-static int tail_reserve(rafting_engine* e, Blk& scratch) {
-    TailLayout L;
-    if (int rc = tail_layout(e->G, L)) return rc;
-    return blk_reserve(scratch, L.total, false);
-}
 
-// Enqueues the tail selection on the engine's stream: list[0 .. n_host) is the host's part (device copy), the tail goes to
-// list[n_host .. n_host + cap), the due total to *n_due.  scratch holds tail_layout(G).total bytes.
-static int tail_select(rafting_engine* e, uint8_t* scratch, int64_t until, uint32_t* list, uint32_t n_host, uint32_t cap, uint32_t* n_due) {
+// Enqueues the selection on the engine's stream: the groups a sweep at `until` fires, except the n_host gids of list (device
+// memory), go to out[0 .. cap) and, when `fill`, the groups that are neither listed nor due after them; the due total goes to
+// *n_due and, unless next is null, the earliest armed deadline after `until` (INT64_MAX: none) to *next.  scratch holds L.total
+// bytes, L = due_layout(G).
+static int due_select(rafting_engine* e, const DueLayout& L, uint8_t* scratch, int64_t until, const uint32_t* list, uint32_t n_host,
+                      uint32_t* out, uint32_t cap, bool fill, uint32_t* n_due, int64_t* next) {
     using namespace rafting;
-    TailLayout L;
-    if (int rc = tail_layout(e->G, L)) return rc;
-    uint32_t* member = (uint32_t*)(scratch + L.member); uint32_t* mask = (uint32_t*)(scratch + L.mask);
-    uint64_t* agg = (uint64_t*)(scratch + L.agg); uint64_t* off = (uint64_t*)(scratch + L.off);
-    CU(cudaMemsetAsync(member, 0, (size_t)L.nblocks * TAIL_WARPS * 4, e->stream));
-    if (n_host) tail_member_kernel<<<(n_host + 255u) / 256u, 256, 0, e->stream>>>(list, n_host, member);
-    tail_scan_kernel<<<L.nblocks, DUE_TPB, 0, e->stream>>>(e->T, until, member, mask, agg);
+    uint32_t* member = nullptr;
+    if (n_host) {
+        member = (uint32_t*)(scratch + L.member);
+        CU(cudaMemsetAsync(member, 0, (size_t)L.nblocks * DUE_WARPS * 4, e->stream));
+        due_member_kernel<<<(n_host + 255u) / 256u, 256, 0, e->stream>>>(list, n_host, member);
+    }
+    uint32_t* mask = (uint32_t*)(scratch + L.mask); DueAgg* agg = (DueAgg*)(scratch + L.agg); DueAgg* off = (DueAgg*)(scratch + L.off);
+    auto scan = fill ? due_scan_kernel<true> : due_scan_kernel<false>;
+    auto emit = fill ? due_emit_kernel<true> : due_emit_kernel<false>;
+    scan<<<L.nblocks, DUE_TPB, 0, e->stream>>>(e->T, until, member, mask, agg);
     size_t tb = L.total - L.tmp;
-    CU(cub::DeviceScan::ExclusiveSum(scratch + L.tmp, tb, agg, off, (int)L.nblocks, e->stream));
-    tail_emit_kernel<<<L.nblocks, DUE_TPB, 0, e->stream>>>(mask, agg, off, L.nblocks, list + n_host, cap, n_due);
+    CU(cub::DeviceScan::ExclusiveScan(scratch + L.tmp, tb, agg, off, DueAggOp(), DueAgg{0, 0, I64MAX}, (int)L.nblocks, e->stream));
+    emit<<<L.nblocks, DUE_TPB, 0, e->stream>>>(mask, agg, off, L.nblocks, out, cap, n_due, next);
     CU(cudaGetLastError());
     return RAFTING_OK;
 }
 
 // One query slot: device scratch, a pinned (so mapped) block for the result (and the list when the caller's buffer is not mapped)
 struct DueSlot {
-    Blk dev;                                               // mask, block pairs, their scan, CUB's scratch
+    Blk dev;                                               // due_layout(G).total bytes
     Blk host;                                              // DueResult, then the staged list
     cudaEvent_t ev = nullptr;
     bool inflight = false;
@@ -228,13 +193,9 @@ extern "C" int rafting_timers_due_begin(rafting_engine_t* e, uint32_t slot, int6
     DueSlot& S = e->due->slot[slot];
     if (S.inflight) return fail(RAFTING_E_BUSY, "due-query slot %u has a query in flight", slot);
     if (!S.ev) CU(cudaEventCreateWithFlags(&S.ev, cudaEventDisableTiming));
-    const uint32_t nblocks = (e->G + DUE_TPB - 1) / DUE_TPB;
-    size_t scan_tmp = 0;
-    CU(cub::DeviceScan::ExclusiveScan(nullptr, scan_tmp, (DueAgg*)nullptr, (DueAgg*)nullptr, DueAggOp(), DueAgg{0, 0, I64MAX}, (int)nblocks));
-    Carve c;
-    const size_t o_mask = c.take((size_t)nblocks * (DUE_TPB / 32) * 4), o_agg = c.take((size_t)nblocks * sizeof(DueAgg));
-    const size_t o_off = c.take((size_t)nblocks * sizeof(DueAgg)), o_tmp = c.o;
-    if (int rc = blk_reserve(S.dev, o_tmp + scan_tmp, false)) return rc;
+    DueLayout L;
+    if (int rc = due_layout(e->G, L)) return rc;
+    if (int rc = blk_reserve(S.dev, L.total, false)) return rc;
     // the caller's buffer, if the device can write it (mapped pinned memory); else the slot's staging block
     void* dst = nullptr;
     bool staged = false;
@@ -247,12 +208,8 @@ extern "C" int rafting_timers_due_begin(rafting_engine_t* e, uint32_t slot, int6
     uint8_t* hdev = nullptr;
     CU(cudaHostGetDevicePointer((void**)&hdev, S.host.p, 0));
     if (staged) dst = hdev + 256;
-    uint32_t* mask = (uint32_t*)(S.dev.p + o_mask); DueAgg* agg = (DueAgg*)(S.dev.p + o_agg); DueAgg* off = (DueAgg*)(S.dev.p + o_off);
-    due_scan_kernel<<<nblocks, DUE_TPB, 0, e->stream>>>(e->T, until_ms, mask, agg);
-    size_t tb = scan_tmp;
-    CU(cub::DeviceScan::ExclusiveScan(S.dev.p + o_tmp, tb, agg, off, DueAggOp(), DueAgg{0, 0, I64MAX}, (int)nblocks, e->stream));
-    due_emit_kernel<<<nblocks, DUE_TPB, 0, e->stream>>>(mask, agg, off, nblocks, (uint32_t*)dst, cap, (DueResult*)hdev);
-    CU(cudaGetLastError());
+    DueResult* res = (DueResult*)hdev;
+    if (int rc = due_select(e, L, S.dev.p, until_ms, nullptr, 0, (uint32_t*)dst, cap, false, &res->n_due, &res->next)) return rc;
     CU(cudaEventRecord(S.ev, e->stream));
     S.user = gids_out; S.cap = cap; S.staged = staged;
     S.inflight = true;

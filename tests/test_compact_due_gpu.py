@@ -7,6 +7,8 @@ tail the device chooses right before the step.
     positions; the due lists are smaller than the pipelining rule's lists at d = 3
   * the config #3 storm at R = 5, flags 1 and 5, with caps below and above counts[3]: the tail and counts[3] equal the model
     over rafting_state_export_bulk, and the step equals rafting_step_begin_compact_sweep over the explicit list gids u tail
+  * a due query and a due step over an empty host list, in flight in the same slot number on one state: the tail is the
+    query's list (cut at cap, or followed by fillers) and counts[3] its n_due
   * refusals leave the slot free; the native runs through the stand-in JNIEnv"""
 import ctypes as C
 from collections import deque
@@ -203,6 +205,44 @@ def test_due_step_equals_the_sweep_step_over_its_list_on_the_storm(flags):
         assert np.array_equal(e.digest(0, G), ref.digest(0, G)), f"state after step {k}"
         prev = active.carry_outbox(got, L, A, G)
     assert seen_over >= 1 and seen_under >= 3, (seen_over, seen_under)   # the storm's first sweep holds most of its timeouts
+
+
+def test_due_step_tail_is_the_due_query_list():
+    """A due query and a due step over an empty host list, begun back to back in the same slot number, see one state: the
+    query's list and next deadline equal the model's, counts[3] equals the query's n_due, and the tail is the query's first
+    cap gids (cap below n_due), or the query's whole list followed by fillers (cap above it).  G is not a multiple of the
+    selection's 256-group block."""
+    G, R, rows = 5000, 3, 2
+    F = R - 1
+    cfg = abi.make_cfg(replicas=R, max_groups=G, max_rows=rows, entry_pool_cap=16)
+    init = harness.init_array(G)
+    init["rand_ms"] = 1 + np.random.default_rng(7).integers(0, 1000, G)      # followers' deadlines spread over 1 s
+    e = engine.Engine(cfg)
+    e.open_bulk(0, init)
+    until = int(np.percentile(_table_bulk(e, G)["timer"], 40))
+    ib = abi.Inbox(rows, G, F, with_ops=False, with_events=False, sweep=True)
+    ib.row_now[0] = until
+    host, q = np.zeros(0, np.uint32), np.zeros(G, np.uint32)
+
+    def query_and_step(slot, cap_of):
+        t = _table_bulk(e, G)
+        want = np.flatnonzero(tm.due(t, until))
+        cap = cap_of(len(want))
+        ci = compact.encode_inbox(compact.due_inbox(tm.slice_inbox(ib, host), cap), None, None, sweep=True)
+        cout = compact.CompactOutbox(rows, cap, F, esc_cap=rows * cap * F + 2 * rows * cap)
+        e.timers_due_begin(slot, until, q)
+        e.step_begin_compact_due(slot, host, cap, ci.sweep, ci.as_c(), None, cout.as_c())
+        tail = e.step_wait_compact_due(slot)
+        n_q, nxt = e.timers_due_wait(slot)
+        assert n_q == len(want) and np.array_equal(q[:n_q], want), f"slot {slot}: the query's list"
+        assert nxt == tm.next_deadline(t, until), f"slot {slot}: the query's next deadline"
+        assert int(cout.counts[3]) == n_q and np.array_equal(tail, dm.tail(t, host, cap, until)[0]), f"slot {slot}: the tail"
+        return q[:n_q].copy(), tail
+
+    Q, tail = query_and_step(1, lambda n: n // 3)                       # the step fires a third of the due groups
+    assert len(Q) > 300 and np.array_equal(tail, Q[:len(tail)])
+    Q, tail = query_and_step(2, lambda n: n + 100)                      # ... and this one the rest
+    assert len(Q) > 200 and np.array_equal(tail[:len(Q)], Q) and not np.isin(tail[len(Q):], Q).any()
 
 
 def test_refusals_leave_the_slot_free():

@@ -1,4 +1,5 @@
-"""The register / shared-memory budget of the R = 3 leader-stream kernel, read from the built library (no GPU needed).
+"""The register / shared-memory budget of the R = 3 leader-stream kernel, and the due selection's stack, read from the built
+library (no GPU needed).
 
 pair_kernel<3> runs 128-thread blocks.  At 64 registers, 8 blocks fill one SM's 65 536 registers, and 8 blocks per SM put
 config #2's 64 K groups x 2 follower lanes in one wave on an H100's 132 SMs (DESIGN.md §5).  Each block also takes a
@@ -36,3 +37,17 @@ def test_pair_kernel_keeps_one_wave():
     assert BLOCKS_PER_SM * (r["SHARED"] + RING) <= SMEM_PER_SM, \
         f"pair_kernel<3>: {BLOCKS_PER_SM} x ({r['SHARED']} B static + {RING} B ring) exceeds {SMEM_PER_SM} B of shared memory per SM"
     assert r["STACK"] <= MAX_STACK, f"pair_kernel<3>'s stack frame grew to {r['STACK']} B (was {MAX_STACK})"
+
+
+@pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not installed")
+def test_due_selection_kernels_use_no_stack():
+    """The due query and a due step's tail run these three kernels over every group of the shard: a stack frame or a spill
+    would add local-memory traffic to a pass that reads 16 B per group."""
+    from rafting_b200 import _build
+    out = subprocess.run([CUOBJDUMP, "-res-usage", _build.build()], capture_output=True, text=True, check=True).stdout
+    for kernel in ("due_member_kernel", "due_scan_kernel", "due_emit_kernel"):    # each instantiation, with and without fillers
+        found = re.findall(r"Function (\S*" + kernel + r"\S*):\s*\n\s*(REG:.*)", out)
+        assert found, f"{kernel} not found in cuobjdump -res-usage"
+        for name, usage in found:
+            r = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", usage)}
+            assert r["STACK"] == 0 and r["LOCAL"] == 0, f"{name}: {r['STACK']} B of stack, {r['LOCAL']} B of local memory"
