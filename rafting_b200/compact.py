@@ -148,11 +148,13 @@ def inbox_in_block(block: np.ndarray, in_off, ci: CompactInbox) -> CompactInbox:
 
 
 def _encode_requests(ib: abi.Inbox, ok: np.ndarray, base: np.ndarray, elections: bool = False) -> tuple[CompactRequests, np.ndarray]:
-    """The request list of a dense inbox: every op other than a SUBMIT / TIMEOUT without a draw, in slot order.  Returns it
-    and the mask of the slots it carries (op_c leaves them NONE).  elections: PreVote / RequestVote become records too."""
+    """The request list of a dense inbox: every op other than a SUBMIT / TIMEOUT without a draw whose time fits op_c's 16-bit
+    offset from the row base, in slot order.  Returns it and the mask of the slots it carries (op_c leaves them NONE).
+    elections: PreVote / RequestVote become records too."""
     rows, n = ib.rows, ib.n
     draw = ib.op_nr["y"]
-    listed = (ok != 0) & (((ok != abi.OP_SUBMIT) & (ok != abi.OP_TIMEOUT)) | (draw != 0))
+    far = ib.op_nr["x"] - base[:, None] > 0xFFFF                                # an op escape carries the time in full
+    listed = (ok != 0) & (((ok != abi.OP_SUBMIT) & (ok != abi.OP_TIMEOUT)) | (draw != 0) | far)
     at = np.flatnonzero(listed.reshape(-1))
     if len(at) == 0:
         return CompactRequests(), listed
@@ -231,6 +233,24 @@ def _without_sweep_row_ops(ib: abi.Inbox, on: np.ndarray) -> abi.Inbox:
     return out
 
 
+def stands_for(ib: abi.Inbox, sweep: bool = False) -> abi.Inbox:
+    """The dense inbox a compact step encoded from ib (encode_inbox(ib, ..., sweep=sweep)) stands for: with sweep, the group
+    ops of the sweep rows dropped (the step ignores them there); and in a step flagged RAFTING_INBOX_NO_REQUESTS, every
+    inbound request turned into an op of kind RAFTING_COP_MALFORMED, which the step refuses with BAD_EVENT as it refuses a
+    request the inbox promised not to hold.  The compact step sets that flag itself, exactly when it has no request list."""
+    col = sweep_column(ib) if sweep else np.zeros(ib.rows, np.int64)
+    if ib.op_meta is not None and (col != 0).any():
+        ib = _without_sweep_row_ops(ib, col != 0)
+    if ib.op_meta is None or not ib.flags & abi.INBOX_NO_REQUESTS:
+        return ib
+    out = abi.Inbox.__new__(abi.Inbox)
+    out.__dict__.update(ib.__dict__)
+    kind = ib.op_meta & U64(0xFF)
+    out.op_meta = np.where(kind > U64(abi.OP_TIMEOUT), (ib.op_meta & ~U64(0xFF)) | U64(abi.COP_MALFORMED), ib.op_meta)
+    out.flags = ib.flags & ~abi.INBOX_NO_REQUESTS
+    return out
+
+
 def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray | None, sent_inc: np.ndarray | None = None,
                  elections: bool = False, ballot_term: np.ndarray | None = None, ballot_inc: np.ndarray | None = None,
                  ballot_tags: np.ndarray | None = None, sweep: bool = False) -> CompactInbox:
@@ -250,17 +270,15 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     ballot_tags[r, i, f] (CompactOutbox.ballot_tags() of the step that emitted the ballot; None = no compact ballot, every
     vote reply travels in full).  ballot_term[r, i] / ballot_inc[r, i]: the term and the asking incarnation of the ballot the
     vote replies in (r, i) answer (the decoded ballot columns of that step); a reply whose incarnation differs travels in
-    full.
+    full.  Both may also be given per lane slot [r, i, f], for a pump whose replies answer ballots of different steps.
     sweep: the inbox of a step begun with rafting_step_begin_compact_sweep.  `.sweep` holds ib.row_now (sweep_column), and the
     group ops of the sweep rows are dropped: the step ignores them there, and a request record on a sweep row is refused.
     Off (the default), row_now is not encoded: the compact step has no sweep rows."""
-    if sweep:
-        col = sweep_column(ib)
-        if ib.op_meta is not None and (col != 0).any():
-            ib = _without_sweep_row_ops(ib, col != 0)
-        c = encode_inbox(ib, tags, sent_term, sent_inc, elections, ballot_term, ballot_inc, ballot_tags)
-        c.sweep = col
+    if sweep:                                                 # the inbox the step stands for, and its sweep column
+        c = encode_inbox(stands_for(ib, sweep=True), tags, sent_term, sent_inc, elections, ballot_term, ballot_inc, ballot_tags)
+        c.sweep = sweep_column(ib)
         return c
+    ib = stands_for(ib)                                       # a step promised no requests: those it holds are refused
     rows, n, F = ib.rows, ib.n, ib.F
     c = CompactInbox(rows, n, F, gids=ib.gids)
     ek = (ib.ev_meta & U64(0xF)).astype(np.int64) if ib.ev_meta is not None else np.zeros((rows, n, F), np.int64)
@@ -283,7 +301,7 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
         if (dt < 0).any() or (dt > 0xFFFF).any():
             raise ValueError("a group op lies more than 65.535 s after its row's base time: use the dense path for this step")
         unav = ib.op_ab["x"].astype(np.uint64) if ib.op_ab is not None else np.zeros((rows, n), np.uint64)
-        unav[listed] = 0
+        unav[listed | (ok == 0)] = 0                                           # only a SUBMIT / TIMEOUT in op_c has a mask
         if (unav > U64(0xFFFF)).any():
             raise ValueError("unavailable mask beyond 16 lanes")
         count = np.where(listed, U64(0), (ib.op_meta >> U64(16)) & U64(0xFFFF))
@@ -310,8 +328,9 @@ def encode_inbox(ib: abi.Inbox, tags: np.ndarray | None, sent_term: np.ndarray |
     escaped = U64(abi.CEV_ESCAPED)
     if elections:
         is_vote = (ek == abi.EV_PV_REPLY) | (ek == abi.EV_RV_REPLY)
-        bt = (ballot_term if ballot_term is not None else np.zeros((rows, n), np.int64))[:, :, None].astype(np.uint64)
-        binc = (ballot_inc if ballot_inc is not None else np.zeros((rows, n), np.uint64))[:, :, None].astype(np.uint64)
+        lane = lambda a: a if a.ndim == 3 else a[:, :, None]                  # per (row, group), or per lane slot
+        bt = lane(ballot_term if ballot_term is not None else np.zeros((rows, n), np.int64)).astype(np.uint64)
+        binc = lane(ballot_inc if ballot_inc is not None else np.zeros((rows, n), np.uint64)).astype(np.uint64)
         rt = ib.ev_tn["x"].astype(np.uint64)
         is_ok = outcome == abi.OUT_OK
         cterm = np.where(is_ok, bt - rt, U64(0))                                 # modulo 2^64: a higher term wraps past 7

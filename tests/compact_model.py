@@ -6,13 +6,18 @@ around it — TEST INFRASTRUCTURE.
   prev_term_words    the only restatement of the kind-7 rule: what PT changes in a packed outbox
   encode / next_of   what a pump encodes a step's inbox with, and what it keeps from the step for the next one
   Driver             such a pump around the engine, checked against the oracle every step (-m gpu)
+  FuzzPump           harness.Fuzzer's streams through the codec and the model, and the engine with -m gpu, on the matrix
+                     COMPACT_FUZZ (tests/test_compact_fuzz_{cpu,gpu}.py)
 
 The CPU suites (tests/test_compact_*_cpu.py) run the model around the oracle to check that the compact wire format of
 include/rafting_b200.h is lossless without a GPU; under -m gpu the real kernels are checked against the oracle and the
 model (tests/test_compact_*_gpu.py)."""
 from __future__ import annotations
 
+from dataclasses import dataclass
+
 import numpy as np
+import pytest
 
 from oracle import binding
 from rafting_b200 import abi, compact, workload
@@ -314,9 +319,10 @@ def assert_step_reads_the_same(a: abi.Inbox, b: abi.Inbox, where=""):
     """Every inbox column the step reads: lane events where present, and per group op what its kind uses (SUBMIT / TIMEOUT:
     time, draw and unavailable mask; requests: every field, entry terms by value)."""
     ek = (a.ev_meta & U64(0xF)) != 0
+    ok = ek & (((a.ev_meta >> U64(4)) & U64(3)) == abi.OUT_OK)         # a reply's term is read only when it came back OK
     assert np.array_equal(a.ev_meta, b.ev_meta), where
-    for name in ("ev_tn", "ev_el"):
-        assert np.array_equal(getattr(a, name)[ek], getattr(b, name)[ek]), f"{name} {where}"
+    assert np.array_equal(a.ev_tn["y"][ek], b.ev_tn["y"][ek]) and np.array_equal(a.ev_tn["x"][ok], b.ev_tn["x"][ok]), f"ev_tn {where}"
+    assert np.array_equal(a.ev_el[ek], b.ev_el[ek]), f"ev_el {where}"
     lo = lambda m: m & U64(0xFFFFFFFF)
     assert np.array_equal(lo(a.op_meta), lo(b.op_meta)), f"op kind / peer / count {where}"
     kind = (a.op_meta & U64(0xFF)).astype(np.int64)
@@ -465,3 +471,292 @@ class Driver:
             self.records += int((cout.esc[:int(cout.counts[0])]["kind"] == abi.CESC_PLAN).sum())
         self.nxt, self.prev = next_of(want, cout), want
         return cin, want, cout
+
+
+# ---- the fuzz pump: harness.Fuzzer's streams through the compact host path ----
+
+@dataclass(frozen=True)
+class CompactCase(harness.FuzzCase):
+    """A harness.FuzzCase on the compact host path.  n_active: the host's list (tail stays 0: a compact list holds gids below
+    max_groups only); for a due step the device appends up to `cap` more.
+      entry      whole: rafting_step_begin_compact / _req (flags 0) or _ex; active: _active over the list; sweep: _sweep over
+                 the whole shard, active-sweep: over the list; due: _due over the list, one sweep row per step
+      cflags     the compact step's flags (EL, PT)
+      cfg_flags  the engine's cfg.flags
+      esc_step   the step that runs with an escape list of ESC_SMALL records: it overflows, and the dense fetch stands in"""
+    entry: str = "whole"
+    cflags: int = 0
+    cfg_flags: int = 0
+    esc_step: int = 2
+
+    def cfg(self) -> abi.Cfg:
+        return abi.make_cfg(replicas=self.R, local_slot=self.local_slot, max_groups=self.G, max_rows=self.rows,
+                            pre_vote=self.pre_vote, entry_pool_cap=self.rows * self.G * 8, flags=self.cfg_flags)
+
+    @property
+    def listed(self) -> bool:
+        return self.entry in ("active", "active-sweep", "due")
+
+
+def _c(id, R, G, seed, entry, cflags=0, sorted_=False, **kw):
+    sweep = {"sweep": 7, "active-sweep": 5, "due": kw.get("rows", 3)}.get(entry, 0)
+    steps = dict(steps=10, cpu_steps=4, leader_share=0.35, state_every=5) if sorted_ else dict(steps=16, cpu_steps=6, state_every=5)
+    steps.update(kw)
+    return CompactCase(id, R, G, seed, entry=entry, cflags=cflags, sweep_every=sweep, stray=4, **steps)
+
+
+ESC_SMALL = 4
+CFG_BOTH = abi.CFG_STRICT_CANDIDATE_VOTE | abi.CFG_LENIENT_FOLLOWER_COMMIT
+
+# R = 2, 3, 5, 9, 17 (every step kernel the compact path reaches), unsorted (n < 2048) and class-sorted (n >= 2048 with
+# requests, steady leaders elected first), every entry point, the flags spread over the cases, wide values on about half
+COMPACT_FUZZ = [
+    _c("R2-G777-whole", 2, 777, 61, "whole", local_slot=1),
+    _c("R2-active2100-EL-wide", 2, 4096, 62, "active", EL, sorted_=True, n_active=2100, compact=True, wide=True),
+    _c("R3-G777-whole-ELPT-wide", 3, 777, 63, "whole", EL | PT, wide=True),
+    _c("R3-G2304-sweep-PT", 3, 2304, 64, "sweep", PT, sorted_=True, local_slot=1),
+    _c("R3-G777-due", 3, 777, 65, "due", n_active=300, compact=True, local_slot=2),
+    _c("R5-G777-sweep-EL-strict-lenient", 5, 777, 66, "sweep", EL, local_slot=2, cfg_flags=CFG_BOTH),
+    _c("R5-active2100-sweep-ELPT-wide", 5, 4096, 67, "active-sweep", EL | PT, sorted_=True, n_active=2100, compact=True,
+       wide=True, local_slot=4),
+    _c("R9-G600-due-ELPT-wide", 9, 600, 68, "due", EL | PT, n_active=200, compact=True, wide=True, local_slot=8),
+    _c("R9-G2304-whole-PT", 9, 2304, 69, "whole", PT, sorted_=True, local_slot=3),
+    _c("R17-G300-whole-EL-wide", 17, 300, 70, "whole", EL, wide=True),
+    _c("R17-active200-sweep-PT", 17, 300, 71, "active-sweep", PT, n_active=200, compact=True, local_slot=16),
+]
+
+
+class StreamCoverage:
+    """Where a case's stream went, through the codec: per-step launches, roles, reply error codes, event kinds as words and
+    as escape records, kind-7 words, compact ballot lanes, events whose time lay beyond the 16-bit offset of their row, and
+    AppendEntries records of groups whose log lies beyond 2^32 with a leader commit above the group's own (wide_records:
+    the record's prev + d_commit then moves the follower's commit index).
+    Not among them: a (group, follower) lane with all 32 tags in flight.  A leader keeps at most IN_FLIGHT_LIMIT = 20 RPCs
+    in flight per follower (Leadership.java:11), and in these streams a lane holds at most 21 busy tags; a lane runs out
+    only when leaders step down and are elected again while their old tags go unanswered (tests/test_group_edit_gpu.py
+    reaches it through reopened gids)."""
+
+    def __init__(self):
+        self.launches, self.roles, self.errs = set(), set(), set()
+        self.words, self.escaped = set(), set()
+        self.kind7 = self.ballot_lanes = self.far = self.wide_records = self.overflows = self.due_over = self.due_under = 0
+
+
+class FuzzPump:
+    """harness.Fuzzer's inboxes through the compact host path, against the oracle stepping the dense inbox into a poisoned
+    outbox.  Every step:
+      * the dense inbox is encoded (compact.encode_inbox) and the model's unpack must read it the same
+        (assert_step_reads_the_same), over the model's own in-flight table;
+      * the model's pack of the oracle's outbox, decoded, must equal that outbox;
+      * with an engine (-m gpu), the engine steps the compact inbox through the case's entry point, and (a) its decoded
+        outbox equals the oracle's, (b) its raw outbox equals the model's pack word for word, (c) under PT an unflagged twin
+        engine's outbox through prev_term_words equals it, (d) a spread of groups' state equals the oracle's every
+        state_every steps, every group's at the end.
+    A reply the fuzz sends may answer a plan of any earlier step and row, so the pump finds the tag each reply echoes in the
+    model's in-flight table (the lowest busy tag of the lane whose parked echo pair and incarnation match; under EL a ballot
+    tag of the reply's incarnation for a vote reply) instead of taking the tags of the last step by slot.  A reply that
+    matches no tag, or a forged or stale one, goes in as the encoder decides."""
+
+    def __init__(self, case: CompactCase, engine: bool = False):
+        self.case, self.cfg = case, case.cfg()
+        G, F = case.G, case.R - 1
+        self.G, self.F, self.rows = G, F, case.rows
+        self.ref = harness.OracleSUT(self.cfg)
+        init = case.init()
+        self.ref.open_bulk(0, init)
+        self.e = self.twin = None
+        if engine:
+            from rafting_b200 import engine as eng
+            self.e = eng.Engine(self.cfg)
+            self.e.open_bulk(0, init)
+            if case.cflags & PT:
+                self.twin = eng.Engine(self.cfg)
+                self.twin.open_bulk(0, init)
+        self.st = InFlight(G, F)
+        self.ballot = np.zeros((CTAGS, G, F), bool)                 # the tag parks a ballot (EL), not an AE / IS plan
+        states = [self.ref.export(g) for g in range(G)]
+        self.term = np.array([s.current_term for s in states], np.int64)
+        self.inc = np.array([s.incarnation for s in states], np.uint32)
+        self.commit = np.array([s.commit_index for s in states], np.int64)
+        self.out = None
+        if case.leader_share:
+            w1 = workload.make_wl(case.seed, 1, G, F, local_slot=case.local_slot)
+            self.out = harness.elect_all(self.ref, w1)
+            for e in (self.e, self.twin):
+                if e is not None:
+                    harness.assert_outbox_equal(self.out, harness.elect_all(e, w1), where=f"{case.id}: election (dense path)")
+            self.term, self.inc = self.out.current_term.copy(), self.out.incarnation.copy()
+            self.commit = self.out.commit_index.copy()
+        self.gids = case.gids()
+        self.fz = harness.Fuzzer(self.cfg, self.ref, seed=case.seed, rows=case.rows, gids=self.gids,
+                                 leader_share=case.leader_share, sweep_every=case.sweep_every, stray_requests=case.stray,
+                                 t0=harness.T33 if case.wide else 0, jump=40_000 if case.wide else 0, unavail_lanes=F,
+                                 near_commit=case.wide)
+        self.spread = np.arange(0, G, max(1, G // 97))
+        self.cov = StreamCoverage()
+        self.k = 0
+
+    # -- what the pump keeps between steps: the model's in-flight table, and every group's term and incarnation --
+    def answer_tags(self, ib: abi.Inbox, L: np.ndarray) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+        """-> (ack tags, ballot tags, ballot terms, ballot incarnations), [rows, n, F] over the step's positions L"""
+        rows, n, F = ib.rows, ib.n, self.F
+        tags = np.full((rows, n, F), abi.CTAG_NONE, np.uint8)
+        btags = np.full((rows, n, F), abi.CTAG_NONE, np.uint8)
+        bterm, binc = np.zeros((rows, n, F), np.int64), np.zeros((rows, n, F), np.uint64)
+        ek = (ib.ev_meta & U64(0xF)).astype(np.int64)
+        taken = {}
+        el = bool(self.case.cflags & EL)
+        for r, i, f in np.argwhere(ek != 0):                        # row-major: a lane's events in row order
+            g, kind = int(L[i]), int(ek[r, i, f])
+            vote = kind in (abi.EV_PV_REPLY, abi.EV_RV_REPLY)
+            if vote and not el:
+                continue
+            busy = int(self.st.bits[g, f]) & ~taken.get((g, f), 0)
+            inc = int(ib.ev_meta[r, i, f] >> U64(32))
+            for t in range(CTAGS):
+                if not (busy >> t) & 1 or int(self.st.inc[t, g, f]) != inc or bool(self.ballot[t, g, f]) != vote:
+                    continue
+                if vote:
+                    btags[r, i, f], bterm[r, i, f], binc[r, i, f] = t, int(self.st.el[t, g, f]["x"]), inc
+                elif (int(self.st.el[t, g, f]["x"]), int(self.st.el[t, g, f]["y"])) == (int(ib.ev_el[r, i, f]["x"]), int(ib.ev_el[r, i, f]["y"])):
+                    tags[r, i, f] = t
+                else:
+                    continue
+                taken[(g, f)] = taken.get((g, f), 0) | (1 << t)
+                break
+        return tags, btags, bterm, binc
+
+    def _pack(self, want: abi.Outbox, L, cap: int, replies: bool) -> compact.CompactOutbox:
+        from tests import compact_active_model as active
+        return active.pack(want, oracle_epoch(self.ref.o, self.G), self.st, cap, flags=self.case.cflags, replies=replies, gids=L)
+
+    def step(self):
+        from tests import compact_active_model as active
+        from tests import due_model as dm
+        from tests import launch_model
+        from tests import timers_model as tm
+        case, G, F, rows, k, cov = self.case, self.G, self.F, self.rows, self.k, self.cov
+        flags, where = case.cflags, f"{case.id}: step {k}"
+        ib = self.fz.make(self.out)
+        if case.listed:
+            ib.flags |= abi.INBOX_COMPACT_GROUPS
+        sweep = case.entry in ("sweep", "active-sweep", "due")
+        cap = 0
+        if case.entry == "due":
+            until = int(ib.row_now.max())
+            t = tm.table([self.ref.export(g) for g in range(G)])
+            n_due = len(np.setdiff1d(np.flatnonzero(tm.due(t, until)), self.gids))
+            cap = min(max(1, n_due // 2) if k % 2 else n_due + 3, G - len(self.gids))
+            tail, self.n_due = dm.tail(t, self.gids, cap, until)
+            cov.due_over += self.n_due > cap; cov.due_under += self.n_due <= cap
+            ib = compact.due_inbox(ib, cap)
+            L = np.concatenate([self.gids, tail]).astype(np.uint32)
+        else:
+            L = self.gids if case.listed else None
+        pos = np.arange(G) if L is None else L.astype(np.int64)
+        n = ib.n
+        # the reference: the oracle steps the dense inbox (a due step over gids u tail, positional)
+        ri = ib
+        if case.entry == "due":
+            ri = abi.Inbox.__new__(abi.Inbox); ri.__dict__.update(ib.__dict__); ri.gids = L
+        want = self.ref.step(ri)
+        # encode; the model's unpack reads what the step reads
+        tags, btags, bterm, binc = self.answer_tags(ib, pos)
+        ci = compact.encode_inbox(ib, tags, self.term[pos], self.inc[pos], elections=bool(flags & EL), ballot_term=bterm,
+                                  ballot_inc=binc, ballot_tags=btags, sweep=sweep)
+        if k % 2 == 0 and ci.reqs is None:
+            ci.reqs = compact.CompactRequests()                       # an empty list: replies may travel in rep_c
+        seen = compact.stands_for(ib, sweep)
+        assert_step_reads_the_same(seen, active.unpack(ci, self.term, self.st, flags, gids=L), where=f"encode -> unpack, {where}")
+        big = rows * n * F + 2 * rows * n
+        cap_out = ESC_SMALL if k == case.esc_step else big
+        mco = self._pack(want, L, cap_out, replies=ci.reqs is not None)
+        if int(mco.counts[0]) > cap_out:
+            cov.overflows += 1
+            with pytest.raises(OverflowError):
+                compact.decode_outbox(mco, elections=bool(flags & EL), prev_term=bool(flags & PT))
+        else:
+            harness.assert_outbox_equal(want, compact.decode_outbox(mco, elections=bool(flags & EL), prev_term=bool(flags & PT)),
+                                        where=f"pack -> decode, {where}")
+        if self.e is not None:
+            self._engine_step(ib, ci, cap, L, want, mco, cap_out, where)
+        # coverage
+        has_reqs = ci.reqs is not None and (len(ci.reqs.req) or len(ci.reqs.op_esc))
+        cov.launches.add(launch_model.kernels(case.R, n, 0 if has_reqs else abi.INBOX_NO_REQUESTS))
+        grp = np.arange(n) if case.listed else pos
+        cov.roles |= set((want.role_word[grp] & 3).tolist())
+        cov.errs |= set(((want.rep_meta >> np.uint32(8)) & np.uint32(0xFF)).ravel().tolist())
+        cov.words |= set((ci.ev_c & np.uint32(0xF)).ravel().tolist()) - {0, abi.CEV_ESCAPED}
+        cov.escaped |= set((ci.esc["ev_meta"] & U64(0xF)).astype(np.int64).tolist())
+        kinds = mco.plan_c & np.uint32(7)
+        cov.kind7 += int((kinds == abi.CPLAN_AE_PREV_TERM).sum())
+        cov.ballot_lanes += int(((kinds == abi.CPLAN_PREVOTE) | (kinds == abi.CPLAN_VOTE)).sum())
+        ek = (ib.ev_meta & U64(0xF)) != 0
+        cov.far += int((ek & (ib.ev_tn["y"] - ci.row_base[:, None, None] > 0xFFFF)).sum())
+        if ci.reqs is not None and len(ci.reqs.req):
+            q = ci.reqs.req[((ci.reqs.req["meta"] >> np.uint32(11)) & np.uint32(3)) == 0]
+            prev = q["prev_index"].astype(np.int64)
+            lc = prev + q["d_commit"].astype(np.int64)
+            cov.wide_records += int(((prev >= 1 << 32) & (lc > self.commit[pos[q["slot"].astype(np.int64) % n]])).sum())
+        # what the pump keeps
+        kk, tg = mco.plan_c & np.uint32(7), mco.tags()
+        for r in range(rows):
+            at = np.argwhere(tg[r] < CTAGS)
+            self.ballot[tg[r][at[:, 0], at[:, 1]], pos[at[:, 0]], at[:, 1]] = kk[r][at[:, 0], at[:, 1]] >= abi.CPLAN_PREVOTE
+        self.term[pos] = want.current_term[:n] if case.listed else want.current_term
+        self.inc[pos] = want.incarnation[:n] if case.listed else want.incarnation
+        self.commit[pos] = want.commit_index[:n] if case.listed else want.commit_index
+        self.out = want
+        if self.e is not None and k % case.state_every == case.state_every - 1:
+            for e in (self.e, self.twin):
+                if e is not None:
+                    harness.assert_states_equal(self.ref, e, self.spread.tolist(), F, where=where)
+        self.k += 1
+        return want
+
+    def _engine_step(self, ib, ci, cap, L, want, mco, cap_out, where):
+        F, rows, n, flags = self.F, self.rows, ib.n, self.case.cflags
+        el, pt = bool(flags & EL), bool(flags & PT)
+
+        def run(e, fl, esc_cap):
+            cout = compact.CompactOutbox(rows, n, F, esc_cap=esc_cap, gids=None if L is None or self.case.entry == "due" else L)
+            if self.case.entry == "due":
+                e.step_compact_due(ci, cout, cap, reqs=ci.reqs, flags=fl)
+                assert np.array_equal(cout.gids, L), f"the due step's tail differs from the model's, {where}"
+                assert int(cout.counts[3]) == self.n_due, f"counts[3] = {int(cout.counts[3])}, {self.n_due} due, {where}"
+            else:
+                e.step_compact(ci, cout, reqs=ci.reqs, flags=fl)
+            return cout
+
+        cout = run(self.e, flags, cap_out)
+        if int(cout.counts[0]) > cap_out:
+            with pytest.raises(OverflowError):
+                compact.decode_outbox(cout, elections=el, prev_term=pt)
+            dense = abi.Outbox(rows, n, F, n if L is not None else self.G)
+            self.e.step_fetch_dense(0, dense.as_c())
+            harness.assert_outbox_equal(want, dense, where=f"dense fetch after an escape overflow, {where}")
+        else:
+            harness.assert_outbox_equal(want, compact.decode_outbox(cout, elections=el, prev_term=pt), where=f"(a) {where}")
+        # (b) the raw compact outbox against the model's pack of the oracle's outbox
+        assert np.array_equal(cout.plan_c, mco.plan_c), f"(b) plan_c differs from the model, {where}: {np.argwhere(cout.plan_c != mco.plan_c)[:5].tolist()}"
+        assert np.array_equal(cout.rep_c, mco.rep_c), f"(b) rep_c, {where}"
+        assert np.array_equal(cout.tags(), mco.tags()) and np.array_equal(cout.tags(rpc_only=True), mco.tags(rpc_only=True)), where
+        assert np.array_equal(cout.counts[:3], mco.counts[:3]), f"(b) counts {cout.counts} vs {mco.counts}, {where}"
+        if int(cout.counts[0]) <= cap_out:
+            assert _sorted_esc(cout) == _sorted_esc(mco), f"(b) escape records, {where}"
+        if self.twin is not None:                                      # (c)
+            cout0 = run(self.twin, flags & ~PT, rows * n * F + 2 * rows * n)
+            model = prev_term_words(cout0, cap_out)
+            assert np.array_equal(cout.plan_c, model.plan_c), f"(c) plan_c, {where}"
+            assert np.array_equal(cout.counts[:3], model.counts[:3]), f"(c) counts, {where}"
+            if int(cout.counts[0]) <= cap_out:
+                assert _sorted_esc(cout) == _sorted_esc(model), f"(c) escape records, {where}"
+
+    def run(self, steps: int) -> StreamCoverage:
+        for _ in range(steps):
+            self.step()
+        if self.e is not None:
+            for e in (self.e, self.twin):
+                if e is not None:
+                    harness.assert_states_equal(self.ref, e, range(self.G), self.F, where=f"{self.case.id}: end of the run")
+        return self.cov

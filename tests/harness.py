@@ -89,10 +89,16 @@ class Fuzzer:
                       groups elected beforehand (elect_all) stay steady-state leaders
       sweep_every     every k-th row of the stream is a timer sweep row (row_now set), ops and lane events kept
       stray_requests  every k-th step is flagged RAFTING_INBOX_NO_REQUESTS and keeps its requests
-      t0              added to every time the fuzz writes"""
+      t0              added to every time the fuzz writes
+      jump            added to the time at a third and at two thirds of every row, so that the row's last third lies more
+                      than 2 * jump ms after its first position
+      unavail_lanes   SUBMIT / TIMEOUT draw their unavailable mask from that many low bits (default 2)
+      near_commit     an inbound AppendEntries carries a leader commit a few entries above its prevLogIndex and the
+                      group's own commit index, instead of one drawn from [0, last + 3), and most carry no election-timeout
+                      draw: with logs near 2^40 they then fit a compact request record (d_commit an int32, no draw)"""
 
     def __init__(self, cfg: abi.Cfg, ref, seed=1, rows=3, n=None, gids=None, leader_share=0.0, sweep_every=0,
-                 stray_requests=0, t0=0):
+                 stray_requests=0, t0=0, jump=0, unavail_lanes=2, near_commit=False):
         self.cfg, self.ref = cfg, ref
         self.rng = np.random.default_rng(seed)
         self.aux = np.random.default_rng([seed, 0xA5])     # the knobs draw from here, never from rng
@@ -108,6 +114,7 @@ class Fuzzer:
         if leader_share:
             self.steady[self.aux.permutation(self.n)[:int(leader_share * self.n)]] = True
         self.sweep_every, self.stray = sweep_every, stray_requests
+        self.jump, self.unavail, self.near_commit = jump, 1 << unavail_lanes, near_commit
         self.row_count = self.step_count = 0
 
     def gid(self, i: int) -> int:
@@ -149,6 +156,8 @@ class Fuzzer:
                     ib.row_now[r] = self.now + 1
             for i in range(self.n):
                 self.now += 1
+                if self.jump and i in (self.n // 3, 2 * self.n // 3):
+                    self.now += self.jump
                 gid = self.gid(i)
                 if gid >= G:               # takes no part in the step; neither side writes its cells
                     ib.timeout(r, i, self.now)
@@ -163,10 +172,10 @@ class Fuzzer:
                 if u < 0.25:
                     pass
                 elif u < 0.40:
-                    ib.submit(r, i, self.now, count=int(rng.integers(1, 4)), unavail=int(rng.integers(0, 4)) if rng.random() < 0.1 else 0)
+                    ib.submit(r, i, self.now, count=int(rng.integers(1, 4)), unavail=int(rng.integers(0, self.unavail)) if rng.random() < 0.1 else 0)
                 elif u < 0.55:
                     ib.timeout(r, i, self.now, rand=int(rng.integers(900, 1801)) if rng.random() < 0.7 else 0,
-                               unavail=int(rng.integers(0, 4)) if rng.random() < 0.1 else 0)
+                               unavail=int(rng.integers(0, self.unavail)) if rng.random() < 0.1 else 0)
                 elif u < 0.75:
                     # inbound AppendEntries from a plausible leader
                     t = term + int(rng.choice([-1, 0, 0, 0, 1, 2]))
@@ -198,8 +207,12 @@ class Fuzzer:
                         ent.append(min(base_t, max(t, base_t)))
                     first = None if rng.random() < 0.95 else prev + 1 + int(rng.integers(1, 3))
                     peer = st.current_leader if (st.current_leader >= 0 and rng.random() < 0.9) else self._peer()
-                    ib.ae_request(r, i, self.now, peer, t, prev, prev_t, ent, leader_commit=int(rng.integers(0, last + 3)),
-                                  first_index=first, rand=int(rng.integers(900, 1801)))
+                    commit, draw = int(rng.integers(0, last + 3)), int(rng.integers(900, 1801))
+                    if self.near_commit:
+                        commit = max(prev, st.commit_index) + int(self.aux.integers(0, n_ent + 3))
+                        draw = draw if self.aux.random() < 0.3 else 0
+                    ib.ae_request(r, i, self.now, peer, t, prev, prev_t, ent, leader_commit=commit, first_index=first,
+                                  rand=draw)
                 elif u < 0.85:
                     t = term + int(rng.choice([-1, 0, 1, 1, 2]))
                     li = st.last_index + int(rng.integers(-1, 2)) if st.last_index >= st.first_index else st.epoch_index + int(rng.integers(0, 2))
