@@ -828,6 +828,32 @@ int rafting_log_gather_step_begin(rafting_engine_t* e, uint32_t slot /* 0..3 */,
                                   rafting_plan_ref_t* plans_out, uint32_t plans_cap);
 int rafting_log_gather_step_wait (rafting_engine_t* e, uint32_t slot,
                                   uint32_t* n_refs, size_t* bytes, uint32_t* n_plans, uint32_t* host_served);
+/* PAYLOADS OF RANGES, gathered on the device without blocking: rafting_log_gather's arguments and result, split into a begin
+ * and a wait, e.g. for the apply ranges of a step (rafting_outbox_apply_ranges, include/rafting_ingest.h).
+ *   * Result: after the wait, refs_out[0 .. *n_refs) and the blob bytes at each ref's blob_off equal, byte for byte, what
+ *     rafting_log_gather returns for the same arguments at the point in the entry buffer's stream where the begin was enqueued:
+ *     one ref per entry, range after range; len 0xffffffff and term 0 for an entry that was never appended; blob_off 16-byte
+ *     aligned, in ref order, each entry's at the running total of the aligned lengths before it.  *bytes = that total.
+ *   * Tickets: RAFTING_GATHER_TICKETS of them, independent of the step slots; a ticket holds one gather.  A begin on a busy
+ *     ticket is RAFTING_E_BUSY, a wait on an idle one RAFTING_E_INVAL.
+ *   * Checks, all before anything is enqueued: gid >= max_groups, no rafting_log_config, or a null pointer with a non-zero
+ *     count or cap -> RAFTING_E_INVAL; 2^31 entries or more, or more entries than refs_cap -> RAFTING_E_CAPACITY (the ticket
+ *     stays free).  When *bytes exceeds blob_cap the wait returns RAFTING_E_CAPACITY with the bytes needed in *bytes and nothing
+ *     written past blob_cap: begin again with a larger blob.
+ *   * Ordering: the work runs on the entry buffer's stream, behind every rafting_log_append made before the begin; the step
+ *     stream never waits for it.  While any range or step gather is not waited for, rafting_log_append, rafting_log_trim and
+ *     rafting_log_store_open return RAFTING_E_BUSY.  rafting_engine_destroy drains and frees a ticket not waited for.
+ *   * Host work: the begin writes one record per range; the device probes, lays out and copies every entry it holds.  An entry
+ *     the ring does not hold (a newer index in its ring slot, the pinned cold tier, the entry file, trimmed, never appended)
+ *     is served at the wait through the host index; *host_served is their number.  When such an entry has bytes, the wait also
+ *     moves the device-served payloads after it up to their places.
+ *   * Output memory: pinned or registered outputs (blob_out 16-byte aligned) are written by the device directly; any other
+ *     host memory goes through pinned staging of the ticket, copied at the wait.  Outputs stay valid until the wait. */
+#define RAFTING_GATHER_TICKETS 4
+int rafting_log_gather_begin(rafting_engine_t* e, uint32_t ticket /* 0..3 */, uint32_t n_ranges,
+                             const uint32_t* gids, const int64_t* firsts, const uint32_t* counts,
+                             rafting_entry_ref_t* refs_out, uint32_t refs_cap, void* blob_out, size_t blob_cap);
+int rafting_log_gather_wait (rafting_engine_t* e, uint32_t ticket, uint32_t* n_refs, size_t* bytes, uint32_t* host_served);
 int rafting_log_stats (rafting_engine_t* e, uint64_t* out /* appended, head, spilled_bytes, hbm_hits, cold_hits, indexed,
                                                               last gather kernels ns, last gather bytes, trimmed entries,
                                                               cold bytes freed, spills skipped (dead segments) */, uint32_t n);

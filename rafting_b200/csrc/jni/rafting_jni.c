@@ -222,6 +222,27 @@ JNIEXPORT void JNICALL FN(logGatherStepWait)(JNIEnv* env, jclass k, jlong h, jin
     (*env)->ReleaseLongArrayElements(env, result, r, 0);
     if (rc) throw_status(env, rc);
 }
+/* the payloads of (gid, first, count) ranges, e.g. a step's apply ranges, gathered on the device under `ticket` (INTEGRATION.md §7) */
+JNIEXPORT void JNICALL FN(logGatherBegin)(JNIEnv* env, jclass k, jlong h, jint ticket, jint nRanges, jobject gids, jobject firsts,
+                                          jobject counts, jobject refsOut, jint refsCap, jobject blobOut, jlong blobCap) {
+    CHECK(rafting_log_gather_begin(ENG(h), (uint32_t)ticket, (uint32_t)nRanges, (const uint32_t*)BUF(gids), (const int64_t*)BUF(firsts),
+                                   (const uint32_t*)BUF(counts), (rafting_entry_ref_t*)BUF(refsOut), (uint32_t)refsCap, BUF(blobOut),
+                                   (size_t)blobCap));
+}
+/* result = {nRefs, bytes, hostServed}; they are written before RAFTING_E_CAPACITY is thrown, bytes as the bytes needed */
+JNIEXPORT void JNICALL FN(logGatherWait)(JNIEnv* env, jclass k, jlong h, jint ticket, jlongArray result) {
+    if (!result || (*env)->GetArrayLength(env, result) < 3) {
+        jclass c = (*env)->FindClass(env, "java/lang/IllegalArgumentException");
+        if (c) (*env)->ThrowNew(env, c, "logGatherWait: the result array needs 3 elements {nRefs, bytes, hostServed}");
+        return;
+    }
+    uint32_t n = 0, served = 0; size_t bytes = 0;
+    int rc = rafting_log_gather_wait(ENG(h), (uint32_t)ticket, &n, &bytes, &served);
+    jlong* r = (*env)->GetLongArrayElements(env, result, NULL);
+    r[0] = (jlong)n; r[1] = (jlong)bytes; r[2] = (jlong)served;
+    (*env)->ReleaseLongArrayElements(env, result, r, 0);
+    if (rc) throw_status(env, rc);
+}
 JNIEXPORT void JNICALL FN(logTrim)(JNIEnv* env, jclass k, jlong h, jint first, jint count) {
     CHECK(rafting_log_trim(ENG(h), (uint32_t)first, (uint32_t)count, NULL, NULL));
 }

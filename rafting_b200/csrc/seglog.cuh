@@ -69,7 +69,9 @@ struct SegLog {
     std::vector<Floor> floor;                 // [G] host copy of d_floor; gids floor_lo..floor_hi changed since the last upload
     Floor* d_floor = nullptr;
     uint32_t floor_lo = UINT32_MAX, floor_hi = 0;
-    uint32_t step_gathers = 0;                // rafting_log_gather_step_begin calls not waited for
+    uint32_t gathers = 0;                     // step and range gathers begun and not waited for: the host index must stay put
+    ::StepGather* ticket[RAFTING_GATHER_TICKETS] = {};      // rafting_log_gather_begin, created on first use
+    bool ticket_busy[RAFTING_GATHER_TICKETS] = {};
     float last_gather_kernel_ms = 0; uint64_t last_gather_bytes = 0;
 };
 
@@ -244,13 +246,70 @@ __global__ void step_gather_copy_kernel(const GatherReq* __restrict__ req, const
         seglog_gather_entry(req[t >> 3], (uint32_t)(t & 7), ring, K, arena, arena_bytes, oldest_resident, lens + (t >> 3), out);
 }
 
+// ---- the payloads of (gid, first, count) ranges (rafting_log_gather_begin), e.g. the apply ranges of a step ----
+// The host knows the number of entries, and one range may hold 10^5 of them (a group catching up), so every pass runs one
+// thread per entry; the host only writes each range's first ref (an exclusive prefix of the counts).
+//   range_probe_kernel       entry k finds its range, then hit or miss, and the 16-byte-aligned bytes of a hit
+//   (cub scan)               -> each entry's blob offset (device-served bytes before it), miss ordinal and request ordinal
+//   range_emit_kernel        the refs in ref order, one gather request per hit, the miss list
+//   step_gather_copy_kernel  as for the step gather
+struct GRange { int64_t first; uint32_t gid, ref; };     // first index, group, first ref of one range
+struct RangesD { const GRange* r; uint32_t n, N; };       // n ranges, N entries in all
+struct RangeOutD { rafting_entry_ref_t* refs; uint64_t blob_cap; GatherReq* req; uint32_t* miss; };
+
+// the last range whose first ref is <= k (k < N): a range without entries shares its first ref with the next one
+__device__ __forceinline__ uint32_t range_of(const RangesD& s, uint32_t k) {
+    uint32_t lo = 0, hi = s.n;                    // r[lo].ref <= k; every range from hi on starts after k
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (s.r[mid].ref <= k) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// k == N writes the identity, so that the scan's element N is the total
+__global__ void range_probe_kernel(RangesD s, ProbeD d, GAgg* __restrict__ agg) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k > s.N) return;
+    GAgg v = {0, 0, 0};
+    if (k < s.N) {
+        const GRange r = s.r[range_of(s, k)];
+        const uint8_t* rec; uint32_t len;
+        if (step_probe(d, r.gid, r.first + (k - r.ref), rec, len)) { v.a = ((uint64_t)len + 15) & ~15ull; v.c = 1; }
+        else v.b = 1;
+    }
+    agg[k] = v;
+}
+
+// a miss gets the blob offset of the device-served bytes before it; the wait moves what follows a miss the host index holds
+__global__ void range_emit_kernel(RangesD s, ProbeD d, const GAgg* __restrict__ off, RangeOutD o) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= s.N) return;
+    const GRange g = s.r[range_of(s, k)];
+    const GAgg q = off[k];
+    rafting_entry_ref_t r; r.gid = g.gid; r.index = g.first + (k - g.ref); r.blob_off = q.a;
+    const uint8_t* rec; uint32_t len;
+    if (step_probe(d, r.gid, r.index, rec, len)) {
+        r.len = len; r.term = *(const int64_t*)(rec + 16);                                          // SegHdr::term
+        GatherReq w; w.gid = r.gid; w.slot = k; w.index = r.index; w.out_off = q.a;
+        if (q.a + (((uint64_t)len + 15) & ~15ull) > o.blob_cap) w.index = 0;   // past the blob: a request the ring never serves
+        o.req[q.c] = w;
+    } else {
+        r.len = 0xffffffffu; r.term = 0;                                                             // the wait fills them in
+        o.miss[q.b] = k;
+    }
+    o.refs[k] = r;
+}
+
 }  // namespace rafting
 
 using rafting::SegLog; using rafting::SegHdr; using rafting::HostLoc; using rafting::GatherReq; using rafting::AppendRec;
 
+static void gather_free(StepGather*& g);
 static void seglog_release(rafting_engine* e) {
     SegLog* L = e->seglog; if (!L) return;
     if (L->s_log) { cudaStreamSynchronize(L->s_log); cudaStreamDestroy(L->s_log); }
+    for (StepGather*& t : L->ticket) gather_free(t);             // a gather not waited for is drained above, then freed
     if (L->s_spill) { cudaStreamSynchronize(L->s_spill); cudaStreamDestroy(L->s_spill); }
     if (L->ev_tables) cudaEventDestroy(L->ev_tables);
     if (L->ev_log) cudaEventDestroy(L->ev_log);
@@ -390,7 +449,7 @@ static int seglog_spill_for(rafting_engine* e, SegLog* L, uint64_t new_head) {
 static int seglog_wal_put(SegLog* L, const rafting_entry_ref_t* refs, uint32_t n, const uint8_t* blob, std::vector<uint64_t>& file_offs);
 static int log_append_impl(rafting_engine_t* e, const rafting_entry_ref_t* refs, uint32_t n, const void* blob, size_t blob_bytes) {
     if (!e || !e->seglog) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
-    if (e->seglog->step_gathers) return fail(RAFTING_E_BUSY, "a step gather has not been waited for (rafting_log_gather_step_wait)");
+    if (e->seglog->gathers) return fail(RAFTING_E_BUSY, "a gather has not been waited for (rafting_log_gather_wait / _step_wait)");
     if (n == 0) return RAFTING_OK;
     if (!refs || (!blob && blob_bytes)) return fail(RAFTING_E_INVAL, "null argument");
     SegLog* L = e->seglog;
@@ -629,24 +688,32 @@ extern "C" int rafting_log_gather(rafting_engine_t* e, uint32_t n_ranges, const 
 }
 
 // ---- rafting_log_gather_step_begin / _wait: the payloads of the plans of a slot's compact step ----
-// Per slot: device scratch of the passes, and a pinned (so mapped) block for the totals, the miss list and the outputs the
-// device cannot write directly
+// Per slot (and per ticket of rafting_log_gather_begin): device scratch of the passes, and a pinned (so mapped) block for the
+// totals, the miss list and the outputs the device cannot write directly
 struct StepGather {
-    Blk dev;                                   // off1 / off2 aggregates and scans, CUB's scratch, requests, the copy's lens
-    Blk host;                                  // totals (2 x GAgg), miss list [refs_cap], then the staged outputs
+    Blk dev;                                   // aggregates and scans, CUB's scratch, requests, the copy's lens (a range gather: its ranges first)
+    Blk host;                                  // totals (2 x GAgg), miss list [refs_cap], then the staged outputs (a range gather: its ranges last)
     cudaEvent_t ev = nullptr, t0 = nullptr, t1 = nullptr;
-    bool timed = false;                        // the kernels ran (the step has plan columns)
+    bool timed = false;                        // the kernels ran (the step has plan columns, the ranges have entries)
+    bool in_order = false;                     // a range gather: every payload at its place in ref order, host-served ones included
     rafting_entry_ref_t* refs = nullptr; uint32_t refs_cap = 0, plans_cap = 0; uint8_t* blob = nullptr; size_t blob_cap = 0;
     rafting_plan_ref_t* plans = nullptr;
     size_t o_miss = 0, o_refs = 0, o_plans = 0, o_blob = 0;   // offsets in host; the staged outputs only
     bool st_refs = false, st_plans = false, st_blob = false;
 };
-static void step_gather_release(Slot& s) {
-    StepGather* g = s.gather;
+static void gather_free(StepGather*& g) {
     if (!g) return;
     if (g->ev) { cudaEventSynchronize(g->ev); cudaEventDestroy(g->ev); cudaEventDestroy(g->t0); cudaEventDestroy(g->t1); }
     blk_free(g->dev, false); blk_free(g->host, true);
-    delete g; s.gather = nullptr;
+    delete g; g = nullptr;
+}
+static void step_gather_release(Slot& s) { gather_free(s.gather); }
+static int gather_events(StepGather& g) {
+    if (!g.ev) {
+        CU(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
+        CU(cudaEventCreate(&g.t0)); CU(cudaEventCreate(&g.t1));
+    }
+    return RAFTING_OK;
 }
 // the device address of host memory the device can write (pinned or registered, aligned), else null
 static uint8_t* mapped_host(void* p, uintptr_t align) {
@@ -672,10 +739,7 @@ extern "C" int rafting_log_gather_step_begin(rafting_engine_t* e, uint32_t slot,
     CU(cudaSetDevice(e->cfg.device));
     if (!S->gather) S->gather = new StepGather();
     StepGather& g = *S->gather;
-    if (!g.ev) {
-        CU(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
-        CU(cudaEventCreate(&g.t0)); CU(cudaEventCreate(&g.t1));
-    }
+    if (int rc = gather_events(g)) return rc;
     uint8_t* d_refs = mapped_host(refs_out, 8); uint8_t* d_plans = mapped_host(plans_out, 4); uint8_t* d_blob = mapped_host(blob_out, 16);
     g.st_refs = refs_cap && !d_refs; g.st_plans = plans_cap && !d_plans; g.st_blob = blob_cap && !d_blob;
     Carve hc;
@@ -730,7 +794,7 @@ extern "C" int rafting_log_gather_step_begin(rafting_engine_t* e, uint32_t slot,
     }
     CU(cudaEventRecord(g.ev, L->s_log));
     g.refs = refs_out; g.refs_cap = refs_cap; g.blob = (uint8_t*)blob_out; g.blob_cap = blob_cap; g.plans = plans_out; g.plans_cap = plans_cap;
-    S->gathering = true; L->step_gathers++;
+    S->gathering = true; L->gathers++;
     return RAFTING_OK;
 }
 
@@ -756,30 +820,43 @@ static int step_gather_overflow(rafting_engine* e, const Slot& S, uint32_t refs_
     return RAFTING_OK;
 }
 
-extern "C" int rafting_log_gather_step_wait(rafting_engine_t* e, uint32_t slot, uint32_t* n_refs, size_t* bytes, uint32_t* n_plans,
-                                            uint32_t* host_served) {
-    using namespace rafting;
-    if (!e || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
-    Slot* S = e->host ? &e->host->slot[slot] : nullptr;
-    if (!S || !S->gathering) return fail(RAFTING_E_INVAL, "slot %u has no gather in flight", slot);
-    CU(cudaSetDevice(e->cfg.device));
-    SegLog* L = e->seglog; StepGather& g = *S->gather;
-    CU(cudaEventSynchronize(g.ev));
-    S->gathering = false; L->step_gathers--;
-    const GAgg t1 = ((const GAgg*)g.host.p)[0], t2 = ((const GAgg*)g.host.p)[1];   // (refs, plans), (device bytes, misses, hits)
+// A range gather keeps rafting_log_gather's layout, every payload at its place in ref order, but the device laid its payloads
+// out as if no miss had bytes: each ref moves up by the bytes of the host-served entries before it.  Walked from the last ref
+// down to the first such entry, so no payload is overwritten before it has moved.
+static void gather_make_room(StepGather& g, uint64_t n, const uint32_t* miss, uint64_t n_miss, uint64_t shift) {
+    uint64_t m = n_miss;
+    for (uint64_t k = n; shift && k-- > 0;) {
+        rafting_entry_ref_t& r = g.refs[k];
+        if (m && miss[m - 1] == k) {
+            m--;
+            if (r.len != 0xffffffffu) shift -= ((uint64_t)r.len + 15) & ~15ull;
+        } else if (r.len) {
+            memmove(g.blob + r.blob_off + shift, g.blob + r.blob_off, r.len);
+        }
+        r.blob_off += shift;
+    }
+}
+
+// The host side of both waits, after the device's part: staged outputs copied out, the misses served through the host index,
+// the bytes needed, the stats.  t1 = (refs, plans), t2 = (device bytes, misses, hits).  A step gather puts the host-served
+// payloads after the device's; a range gather (g.in_order) puts them where rafting_log_gather does.  S: the step gather's slot,
+// whose refs past refs_cap are sized on the host.
+static int gather_finish(rafting_engine* e, StepGather& g, const rafting::GAgg& t1, const rafting::GAgg& t2, const Slot* S, uint64_t* need_out, bool* fits_out) {
+    SegLog* L = e->seglog;
     if (g.st_refs) memcpy(g.refs, g.host.p + g.o_refs, (size_t)(t1.a < g.refs_cap ? t1.a : g.refs_cap) * sizeof(rafting_entry_ref_t));
     if (g.st_plans) memcpy(g.plans, g.host.p + g.o_plans, (size_t)(t1.b < g.plans_cap ? t1.b : g.plans_cap) * sizeof(rafting_plan_ref_t));
     if (g.st_blob) memcpy(g.blob, g.host.p + g.o_blob, (size_t)(t2.a < g.blob_cap ? t2.a : g.blob_cap));
-    // the misses: lengths and terms from the host index, payloads after the device's
+    // the misses: lengths and terms from the host index
     const uint32_t* miss = (const uint32_t*)(g.host.p + g.o_miss);
     uint64_t need = t2.a;
     for (uint64_t m = 0; m < t2.b; m++) {
         rafting_entry_ref_t& r = g.refs[miss[m]];
-        r.blob_off = need;
+        if (!g.in_order) r.blob_off = need;
         if (const HostLoc* hl = seglog_find(L, r.gid, r.index)) { r.len = hl->len; r.term = hl->term; need += ((uint64_t)hl->len + 15) & ~15ull; }
     }
-    if (t1.a > g.refs_cap) { if (int rc = step_gather_overflow(e, *S, g.refs_cap, &need)) return rc; }
+    if (S && t1.a > g.refs_cap) { if (int rc = step_gather_overflow(e, *S, g.refs_cap, &need)) return rc; }
     const bool fits = t1.a <= g.refs_cap && t1.b <= g.plans_cap && need <= g.blob_cap;
+    if (fits && g.in_order && need > t2.a) gather_make_room(g, t1.a, miss, t2.b, need - t2.a);
     for (uint64_t m = 0; fits && m < t2.b; m++) {
         const rafting_entry_ref_t& r = g.refs[miss[m]];
         if (r.len == 0xffffffffu || r.len == 0) continue;
@@ -789,6 +866,23 @@ extern "C" int rafting_log_gather_step_wait(rafting_engine_t* e, uint32_t slot, 
     if (g.timed) CU(cudaEventElapsedTime(&L->last_gather_kernel_ms, g.t0, g.t1));
     L->last_gather_bytes = need;
     if (fits) L->hbm_hits += t2.c;
+    *need_out = need; *fits_out = fits;
+    return RAFTING_OK;
+}
+
+extern "C" int rafting_log_gather_step_wait(rafting_engine_t* e, uint32_t slot, uint32_t* n_refs, size_t* bytes, uint32_t* n_plans,
+                                            uint32_t* host_served) {
+    using namespace rafting;
+    if (!e || slot >= RAFTING_HOST_SLOTS) return fail(RAFTING_E_INVAL, "bad argument");
+    Slot* S = e->host ? &e->host->slot[slot] : nullptr;
+    if (!S || !S->gathering) return fail(RAFTING_E_INVAL, "slot %u has no gather in flight", slot);
+    CU(cudaSetDevice(e->cfg.device));
+    SegLog* L = e->seglog; StepGather& g = *S->gather;
+    CU(cudaEventSynchronize(g.ev));
+    S->gathering = false; L->gathers--;
+    const GAgg t1 = ((const GAgg*)g.host.p)[0], t2 = ((const GAgg*)g.host.p)[1];   // (refs, plans), (device bytes, misses, hits)
+    uint64_t need; bool fits;
+    if (int rc = gather_finish(e, g, t1, t2, S, &need, &fits)) return rc;
     if (n_refs) *n_refs = (uint32_t)(t1.a < UINT32_MAX ? t1.a : UINT32_MAX);
     if (bytes) *bytes = (size_t)need;
     if (n_plans) *n_plans = (uint32_t)(t1.b < UINT32_MAX ? t1.b : UINT32_MAX);
@@ -799,13 +893,115 @@ extern "C" int rafting_log_gather_step_wait(rafting_engine_t* e, uint32_t slot, 
     return RAFTING_OK;
 }
 
+// ---- rafting_log_gather_begin / _wait: the payloads of (gid, first, count) ranges, rafting_log_gather's result without a
+// host lookup per entry and without blocking the caller between the two calls ----
+extern "C" int rafting_log_gather_begin(rafting_engine_t* e, uint32_t ticket, uint32_t n_ranges, const uint32_t* gids,
+                                        const int64_t* firsts, const uint32_t* counts, rafting_entry_ref_t* refs_out,
+                                        uint32_t refs_cap, void* blob_out, size_t blob_cap) {
+    using namespace rafting;
+    if (!e || ticket >= RAFTING_GATHER_TICKETS || (n_ranges && (!gids || !firsts || !counts)) || (refs_cap && !refs_out) ||
+        (blob_cap && !blob_out))
+        return fail(RAFTING_E_INVAL, "bad argument");
+    if (!e->seglog) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
+    SegLog* L = e->seglog;
+    if (L->ticket_busy[ticket]) return fail(RAFTING_E_BUSY, "ticket %u holds a gather that has not been waited for", ticket);
+    uint64_t N = 0;
+    for (uint32_t r = 0; r < n_ranges; r++) {
+        if (gids[r] >= e->G) return fail(RAFTING_E_INVAL, "range %u: gid out of range", r);
+        N += counts[r];
+    }
+    if (N >= 0x80000000ull) return fail(RAFTING_E_CAPACITY, "%llu entries: a range gather takes fewer than 2^31", (unsigned long long)N);
+    if (N > refs_cap) return fail(RAFTING_E_CAPACITY, "the ranges hold %llu entries, refs_out %u", (unsigned long long)N, refs_cap);
+    CU(cudaSetDevice(e->cfg.device));
+    if (!L->ticket[ticket]) L->ticket[ticket] = new StepGather();
+    StepGather& g = *L->ticket[ticket];
+    if (int rc = gather_events(g)) return rc;
+    g.in_order = true;
+    uint8_t* d_refs = mapped_host(refs_out, 8); uint8_t* d_blob = mapped_host(blob_out, 16);
+    g.st_refs = N && !d_refs; g.st_plans = false; g.st_blob = blob_cap && !d_blob;
+    Carve hc;
+    hc.take(2 * sizeof(GAgg));
+    g.o_miss = hc.take((size_t)N * 4);
+    g.o_refs = g.st_refs ? hc.take((size_t)N * sizeof(rafting_entry_ref_t)) : 0;
+    g.o_plans = 0;
+    g.o_blob = g.st_blob ? hc.take(blob_cap) : 0;
+    const size_t o_ranges_h = hc.take(N ? (size_t)n_ranges * sizeof(GRange) : 0);
+    size_t scan_tmp = 0;
+    if (N) CU(cub::DeviceScan::ExclusiveScan(nullptr, scan_tmp, (GAgg*)nullptr, (GAgg*)nullptr, GAggSum(), GAgg{0, 0, 0}, (int)(N + 1)));
+    Carve dc;
+    const size_t o_ranges = dc.take((size_t)n_ranges * sizeof(GRange));
+    const size_t o_agg = dc.take((N + 1) * sizeof(GAgg)), o_off = dc.take((N + 1) * sizeof(GAgg));
+    const size_t o_req = dc.take(N * sizeof(GatherReq)), o_lens = dc.take(N * 4), o_tmp = dc.take(scan_tmp);
+    int rc;
+    if ((rc = blk_reserve(g.host, hc.o, true)) || (N && (rc = blk_reserve(g.dev, dc.o, false)))) return rc;
+    uint8_t* hdev = nullptr;
+    CU(cudaHostGetDevicePointer((void**)&hdev, g.host.p, 0));
+    if (!d_refs && g.st_refs) d_refs = hdev + g.o_refs;
+    if (!d_blob && g.st_blob) d_blob = hdev + g.o_blob;
+    if ((rc = seglog_floor_flush(L))) return rc;
+    ((GAgg*)g.host.p)[0] = GAgg{N, 0, 0};
+    g.timed = N != 0;
+    if (N) {
+        // each range's first ref, an exclusive prefix of the counts: the one pass over the ranges, none over their entries
+        GRange* hr = (GRange*)(g.host.p + o_ranges_h);
+        uint32_t ref = 0;
+        for (uint32_t r = 0; r < n_ranges; r++) { hr[r].first = firsts[r]; hr[r].gid = gids[r]; hr[r].ref = ref; ref += counts[r]; }
+        GRange* dr = (GRange*)(g.dev.p + o_ranges);
+        GAgg* agg = (GAgg*)(g.dev.p + o_agg); GAgg* off = (GAgg*)(g.dev.p + o_off);
+        RangesD rs; rs.r = dr; rs.n = n_ranges; rs.N = (uint32_t)N;
+        ProbeD pd; pd.ring = L->ring; pd.K = L->K; pd.arena = L->arena; pd.arena_bytes = (uint64_t)L->seg_bytes * L->nseg;
+        pd.oldest = seglog_oldest_resident(L); pd.floor = L->d_floor;
+        RangeOutD od; od.refs = (rafting_entry_ref_t*)d_refs; od.blob_cap = blob_cap; od.req = (GatherReq*)(g.dev.p + o_req);
+        od.miss = (uint32_t*)(hdev + g.o_miss);
+        const uint32_t blocks = (uint32_t)((N + 1 + 255) / 256);
+        const uint64_t copy_blocks = (N * 8 + 255) / 256;
+        CU(cudaMemcpyAsync(dr, hr, (size_t)n_ranges * sizeof(GRange), cudaMemcpyHostToDevice, L->s_log));
+        CU(cudaEventRecord(g.t0, L->s_log));
+        range_probe_kernel<<<blocks, 256, 0, L->s_log>>>(rs, pd, agg);
+        size_t tb = scan_tmp;
+        CU(cub::DeviceScan::ExclusiveScan(g.dev.p + o_tmp, tb, agg, off, GAggSum(), GAgg{0, 0, 0}, (int)(N + 1), L->s_log));
+        range_emit_kernel<<<blocks, 256, 0, L->s_log>>>(rs, pd, off, od);
+        step_gather_copy_kernel<<<(uint32_t)(copy_blocks < 1056 ? copy_blocks : 1056), 256, 0, L->s_log>>>(
+            od.req, off + N, pd.ring, pd.K, pd.arena, pd.arena_bytes, pd.oldest, (uint32_t*)(g.dev.p + o_lens), d_blob);
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(g.t1, L->s_log));
+        CU(cudaMemcpyAsync(g.host.p + sizeof(GAgg), off + N, sizeof(GAgg), cudaMemcpyDeviceToHost, L->s_log));
+    } else {
+        ((GAgg*)g.host.p)[1] = GAgg{0, 0, 0};
+    }
+    CU(cudaEventRecord(g.ev, L->s_log));
+    g.refs = refs_out; g.refs_cap = refs_cap; g.blob = (uint8_t*)blob_out; g.blob_cap = blob_cap; g.plans = nullptr; g.plans_cap = 0;
+    L->ticket_busy[ticket] = true; L->gathers++;
+    return RAFTING_OK;
+}
+
+extern "C" int rafting_log_gather_wait(rafting_engine_t* e, uint32_t ticket, uint32_t* n_refs, size_t* bytes, uint32_t* host_served) {
+    using namespace rafting;
+    if (!e || ticket >= RAFTING_GATHER_TICKETS) return fail(RAFTING_E_INVAL, "bad argument");
+    SegLog* L = e->seglog;
+    if (!L || !L->ticket_busy[ticket]) return fail(RAFTING_E_INVAL, "ticket %u has no gather in flight", ticket);
+    CU(cudaSetDevice(e->cfg.device));
+    StepGather& g = *L->ticket[ticket];
+    CU(cudaEventSynchronize(g.ev));
+    L->ticket_busy[ticket] = false; L->gathers--;
+    const GAgg t1 = ((const GAgg*)g.host.p)[0], t2 = ((const GAgg*)g.host.p)[1];   // (refs, 0), (device bytes, misses, hits)
+    uint64_t need; bool fits;
+    if (int rc = gather_finish(e, g, t1, t2, nullptr, &need, &fits)) return rc;
+    if (n_refs) *n_refs = (uint32_t)t1.a;
+    if (bytes) *bytes = (size_t)need;
+    if (host_served) *host_served = (uint32_t)t2.b;
+    if (!fits)
+        return fail(RAFTING_E_CAPACITY, "ticket %u: the ranges need %llu bytes (blob_cap %zu)", ticket, (unsigned long long)need, g.blob_cap);
+    return RAFTING_OK;
+}
+
 // Garbage collection behind RaftLog.flush (RocksLog.java:228-242: deleteRange below the new epoch): index entries below
 // a group's lowest stored key are dropped, and a cold (pinned host) segment whose last live record went away is freed.
 // A segment with no live record is also never spilled in the first place (seglog_spill_for).
 extern "C" int rafting_log_trim(rafting_engine_t* e, uint32_t first_gid, uint32_t count, uint64_t* dropped_entries, uint64_t* freed_cold_bytes) {
     if (!e || !e->seglog) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
     if ((uint64_t)first_gid + count > e->G) return fail(RAFTING_E_CAPACITY, "gid range beyond max_groups");
-    if (e->seglog->step_gathers) return fail(RAFTING_E_BUSY, "a step gather has not been waited for (rafting_log_gather_step_wait)");
+    if (e->seglog->gathers) return fail(RAFTING_E_BUSY, "a gather has not been waited for (rafting_log_gather_wait / _step_wait)");
     SegLog* L = e->seglog;
     CU(cudaSetDevice(e->cfg.device));
     std::vector<uint64_t> meta(count); std::vector<int64_t> lo(count), hi(count);
@@ -928,7 +1124,7 @@ extern "C" int rafting_log_store_open(rafting_engine_t* e, const char* path, uin
     if (!e || !e->seglog || !path) return fail(RAFTING_E_INVAL, "entry buffer not configured (rafting_log_config)");
     SegLog* L = e->seglog;
     if (L->wal_fd >= 0) return fail(RAFTING_E_INVAL, "entry file already open");
-    if (L->step_gathers) return fail(RAFTING_E_BUSY, "a step gather has not been waited for (rafting_log_gather_step_wait)");
+    if (L->gathers) return fail(RAFTING_E_BUSY, "a gather has not been waited for (rafting_log_gather_wait / _step_wait)");
     if (L->appended) return fail(RAFTING_E_INVAL, "open the entry file before the first append");
     try {
         const int fd = open(path, O_RDWR | O_CREAT, 0644);

@@ -40,7 +40,7 @@ EXPORTS = [
     "rafting_engine_counters", "rafting_abi_sizes", "rafting_checkpoint", "rafting_restore",
     "rafting_step_begin_host", "rafting_step_wait_slot", "rafting_step_begin_compact", "rafting_step_begin_compact_req", "rafting_step_begin_compact_ex", "rafting_step_begin_compact_active", "rafting_step_begin_compact_sweep", "rafting_step_begin_compact_due", "rafting_timers_due_begin", "rafting_timers_due_wait", "rafting_compact_req_layout", "rafting_step_wait_compact", "rafting_step_fetch_dense", "rafting_compact_layout", "rafting_backoff_step", "rafting_allgather_join",
     "rafting_log_config", "rafting_log_append", "rafting_log_read", "rafting_log_gather", "rafting_log_trim", "rafting_log_stats",
-    "rafting_log_gather_step_begin", "rafting_log_gather_step_wait",
+    "rafting_log_gather_step_begin", "rafting_log_gather_step_wait", "rafting_log_gather_begin", "rafting_log_gather_wait",
     "rafting_log_store_open", "rafting_log_sync", "rafting_log_mark", "rafting_log_recovered", "rafting_log_export_kv", "rafting_log_store_stats",
 ]
 
@@ -106,6 +106,10 @@ def lib():
                                                     C.c_void_p, C.c_uint32]
         L.rafting_log_gather_step_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_size_t),
                                                    C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+        L.rafting_log_gather_begin.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_uint32, C.c_void_p, C.c_size_t]
+        L.rafting_log_gather_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_size_t),
+                                              C.POINTER(C.c_uint32)]
         L.rafting_log_trim.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.rafting_log_store_open.argtypes = [C.c_void_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint64)]
         L.rafting_log_sync.argtypes = [C.c_void_p]
@@ -626,6 +630,44 @@ class Engine:
                 refs_cap, blob_cap, plans_cap = max(refs_cap, n), max(blob_cap, b), max(plans_cap, p)
                 continue
             return self._gathered(refs[:n], blob), plans[:p].copy(), h
+
+    GATHER_TICKETS = 4
+
+    def log_gather_begin(self, ticket: int, ranges, refs: np.ndarray, blob: np.ndarray,
+                         refs_cap: int | None = None, blob_cap: int | None = None):
+        """rafting_log_gather_begin: gather, on the entry buffer's stream, the payloads of `ranges` ([(gid, first, count)], or a
+        (gids, firsts, counts) tuple of arrays) under `ticket`.  refs (ENTRY_REF) and blob (uint8) receive what log_gather
+        would return; pinned arrays are written by the device directly.  They must stay alive until log_gather_wait."""
+        for a, dt in ((refs, self.ENTRY_REF), (blob, np.dtype(np.uint8))):
+            if a.dtype != dt or not a.flags.c_contiguous:
+                raise TypeError(f"expected a contiguous {dt} array")
+        if isinstance(ranges, tuple):
+            g, f, c = (np.ascontiguousarray(x, dt) for x, dt in zip(ranges, (np.uint32, np.int64, np.uint32)))
+        else:
+            r = list(ranges)
+            g = np.array([x[0] for x in r], dtype=np.uint32)
+            f = np.array([x[1] for x in r], dtype=np.int64)
+            c = np.array([x[2] for x in r], dtype=np.uint32)
+        rc = len(refs) if refs_cap is None else refs_cap
+        bc = len(blob) if blob_cap is None else blob_cap
+        if rc > len(refs) or bc > len(blob):
+            raise ValueError("a cap beyond its buffer")
+        n = len(g)
+        _check(lib().rafting_log_gather_begin(self._h, ticket, n, g.ctypes.data if n else None, f.ctypes.data if n else None,
+                                              c.ctypes.data if n else None, refs.ctypes.data if len(refs) else None, rc,
+                                              blob.ctypes.data if len(blob) else None, bc), "rafting_log_gather_begin")
+
+    def log_gather_wait(self, ticket: int) -> tuple[int, int, int]:
+        """-> (n_refs, bytes, host_served).  A blob that was too small raises RaftingError (E_CAPACITY) whose `sizes` holds the
+        same tuple, with the bytes needed."""
+        n, b, h = C.c_uint32(), C.c_size_t(), C.c_uint32()
+        rc = lib().rafting_log_gather_wait(self._h, ticket, C.byref(n), C.byref(b), C.byref(h))
+        sizes = (n.value, b.value, h.value)
+        if rc:
+            ex = RaftingError(rc, "rafting_log_gather_wait")
+            ex.sizes = sizes
+            raise ex
+        return sizes
 
     def log_stats(self) -> dict:
         v = np.zeros(11, dtype=np.uint64)

@@ -52,6 +52,9 @@ final class NativeEngine {
     static native void logGatherStepBegin(long h, int slot, ByteBuffer refsOut, int refsCap, ByteBuffer blobOut, long blobCap,
                                           ByteBuffer plansOut, int plansCap);                     // rafting_log_gather_step_begin: a step's AE payloads
     static native void logGatherStepWait(long h, int slot, long[] nRefsBytesNPlansHostServed);   // rafting_log_gather_step_wait
+    static native void logGatherBegin(long h, int ticket, int nRanges, ByteBuffer gids, ByteBuffer firsts, ByteBuffer counts,
+                                      ByteBuffer refsOut, int refsCap, ByteBuffer blobOut, long blobCap);   // rafting_log_gather_begin: ranges' payloads, async
+    static native void logGatherWait(long h, int ticket, long[] nRefsBytesHostServed);           // rafting_log_gather_wait
     static native void logTrim(long h, int first, int count);                                    // rafting_log_trim (behind RaftLog.flush)
     static native int  logRecovered(long h, int gid, ByteBuffer initOut, ByteBuffer runsOut, int cap);   // rafting_log_recovered
     static native void commInitAll(long[] engines);                                              // rafting_comm_init_all: ONE JVM, n shards
