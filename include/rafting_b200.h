@@ -786,6 +786,9 @@ int rafting_log_config(rafting_engine_t* e, uint32_t segment_bytes, uint32_t hbm
 int rafting_log_append(rafting_engine_t* e, const rafting_entry_ref_t* refs, uint32_t n, const void* blob, size_t blob_bytes);
 int rafting_log_read  (rafting_engine_t* e, uint32_t gid, int64_t first_index, uint32_t max_n,
                        rafting_entry_ref_t* refs_out, void* blob_out, size_t blob_cap, uint32_t* n_out);
+/* one ref per entry, range after range; each stored entry's payload at blob_off, the running total of the 16-byte-aligned
+   lengths before it.  *bytes_out = that total, never more than blob_cap: a total beyond blob_cap (aligned lengths, as both
+   device gathers count them) is RAFTING_E_CAPACITY, and so is a total beyond refs_cap entries. */
 int rafting_log_gather(rafting_engine_t* e, uint32_t n_ranges, const uint32_t* gids, const int64_t* firsts,
                        const uint32_t* counts, rafting_entry_ref_t* refs_out, uint32_t refs_cap,
                        void* blob_out, size_t blob_cap, uint32_t* n_out, size_t* bytes_out);

@@ -371,6 +371,13 @@ static inline void seglog_floor(SegLog* L, uint32_t gid, int64_t index, uint64_t
     if (gid < L->floor_lo) L->floor_lo = gid;
     if (gid > L->floor_hi) L->floor_hi = gid;
 }
+// a group's host index starts again from nothing at the record with sequence number seq: every older record of the group is
+// excluded by seq, so the index floor goes back to 0 (left where a trim or cut put it, it would keep the ring from serving
+// every new index below it)
+static inline void seglog_floor_restart(SegLog* L, uint32_t gid, uint64_t seq) {
+    L->floor[gid].index = 0;
+    seglog_floor(L, gid, 0, seq);
+}
 // the changed floors go up on the log stream, ahead of every gather enqueued later (a pageable copy: the host may change them
 // again as soon as this returns)
 static int seglog_floor_flush(SegLog* L) {
@@ -384,17 +391,23 @@ static int seglog_floor_flush(SegLog* L) {
 static inline void seglog_put(SegLog* L, uint32_t gid, int64_t index, const HostLoc& hl, uint64_t seq) {
     rafting::GroupIdx& gi = L->index[gid];
     const HostLoc none = {0, 0xffffffffu, 0, rafting::NO_FILE};
+    // An empty index that starts below its floor (everything was trimmed, then the group's log starts again lower) is a new
+    // window as well.
+    const bool below_floor = gi.v.empty() && index < L->floor[gid].index;
     if (gi.v.empty()) gi.base = index;
     // An index far from everything stored (an InstallSnapshot moved the follower's log, RaftRoutine.java:408-445) starts a
     // new window instead of materialising the gap: what lay on the other side of it is no longer reachable by any plan.
-    if (index < gi.base - SEGLOG_INDEX_WINDOW || index >= gi.base + (int64_t)gi.v.size() + SEGLOG_INDEX_WINDOW) {
+    // Below the window that is any index the newest WINDOW indices would not hold: extending down to it and keeping the
+    // newest window would cut the very index being put.
+    const int64_t end = gi.base + (int64_t)gi.v.size();
+    if (below_floor || index < end - SEGLOG_INDEX_WINDOW || index >= end + SEGLOG_INDEX_WINDOW) {
         for (const HostLoc& h : gi.v) seglog_drop(L, h);
         gi.v.clear(); gi.base = index;
-        seglog_floor(L, gid, 0, seq);                              // every older record of the group is gone
+        seglog_floor_restart(L, gid, seq);                         // every older record of the group is gone
     }
     if (index < gi.base) { gi.v.insert(gi.v.begin(), (size_t)(gi.base - index), none); gi.base = index; }
     if (index >= gi.base + (int64_t)gi.v.size()) gi.v.resize((size_t)(index - gi.base) + 1, none);
-    if (gi.v.size() > (size_t)SEGLOG_INDEX_WINDOW) {                // keep the newest window
+    if (gi.v.size() > (size_t)SEGLOG_INDEX_WINDOW) {                // keep the newest window (index is its newest)
         const size_t cut = gi.v.size() - (size_t)SEGLOG_INDEX_WINDOW;
         for (size_t k = 0; k < cut; k++) seglog_drop(L, gi.v[k]);
         gi.v.erase(gi.v.begin(), gi.v.begin() + (ptrdiff_t)cut); gi.base += (int64_t)cut;
@@ -475,11 +488,14 @@ static int log_append_impl(rafting_engine_t* e, const rafting_entry_ref_t* refs,
         CU(cudaMalloc((void**)&L->d_blob, L->d_blob_cap));
     }
     if (blob_bytes) CU(cudaMemcpyAsync(L->d_blob, blob, blob_bytes, cudaMemcpyHostToDevice, L->s_log));
-    const uint64_t room = (uint64_t)L->seg_bytes * (L->nseg - 1), arena_bytes = (uint64_t)L->seg_bytes * L->nseg;
+    const uint64_t arena_bytes = (uint64_t)L->seg_bytes * L->nseg;
     uint32_t done = 0;
     while (done < n) {
-        // layout pass (arithmetic only): records never straddle a segment; a sub-batch ends where the arena,
-        // minus one segment, would be exceeded
+        // layout pass (arithmetic only): records never straddle a segment; a sub-batch ends before it would reach the arena
+        // slot of the segment that holds L->head, whose records before L->head stay resident.  Counted from that segment's
+        // start, a sub-batch has the whole arena: every segment it overwrites is spilled first, and its first record always
+        // fits, a skipped tail included
+        const uint64_t end = (L->head / L->seg_bytes + L->nseg) * L->seg_bytes;
         const size_t need = (size_t)(n - done) * sizeof(AppendRec);
         if (need > L->stage_cap) {
             CU(cudaStreamSynchronize(L->s_log));
@@ -493,7 +509,7 @@ static int log_append_impl(rafting_engine_t* e, const rafting_entry_ref_t* refs,
             const uint64_t rec = sizeof(SegHdr) + (((uint64_t)refs[i].len + 15) & ~15ull);
             uint64_t h2 = head;
             if (h2 / L->seg_bytes != (h2 + rec - 1) / L->seg_bytes) h2 = (h2 / L->seg_bytes + 1) * L->seg_bytes;   // skip the tail
-            if (h2 + rec - L->head > room) break;
+            if (h2 + rec > end) break;
             AppendRec& r = recs[m];
             r.gid = refs[i].gid; r.len = refs[i].len; r.index = refs[i].index; r.term = refs[i].term; r.loc = h2; r.src = refs[i].blob_off;
             HostLoc hl; hl.off = h2; hl.len = refs[i].len; hl.term = refs[i].term;
@@ -631,7 +647,7 @@ extern "C" int rafting_log_gather(rafting_engine_t* e, uint32_t n_ranges, const 
             o.gid = gids[r]; o.index = idx; o.term = 0; o.blob_off = used; o.len = 0xffffffffu;
             const HostLoc* hl = seglog_find(L, gids[r], idx);      // lengths / offsets come from the host index
             if (hl) {
-                if (used + hl->len > blob_cap) return fail(RAFTING_E_CAPACITY, "blob_out too small");
+                if (used + (((size_t)hl->len + 15) & ~(size_t)15) > blob_cap) return fail(RAFTING_E_CAPACITY, "blob_out too small");
                 o.len = hl->len; o.term = hl->term;
                 if (hl->off != rafting::NO_ARENA && seglog_resident(L, hl->off)) { GatherReq q; q.gid = gids[r]; q.slot = m; q.index = idx; q.out_off = used; req.push_back(q); }
                 else if (hl->len) cold.push_back(m);

@@ -11,22 +11,11 @@ import pytest
 
 from rafting_b200 import abi, compact, engine, workload
 from tests import edit_pump
+from tests.entry_model import dense_ranges
 from tests import harness
 from tests import timers_model as tm
 
 pytestmark = pytest.mark.gpu
-
-
-def dense_ranges(e: engine.Engine, slot: int, rows: int, n: int, gids):
-    """(lane slots, gids, first indices, counts) of the AE plans with entries of the step last waited for in slot"""
-    d = abi.Outbox(rows, n, e.F, n)
-    e.step_fetch_dense(slot, d.as_c())
-    m = d.plan_meta.reshape(-1)
-    c = np.where((m & 0xF) == abi.PLAN_AE, (m >> 16) & 0xFFFF, 0).astype(np.int64)
-    t = np.flatnonzero(c)
-    pos = (t // e.F) % n
-    g = pos if gids is None else np.asarray(gids, np.int64)[pos]
-    return t, g, d.plan_pp.reshape(-1)["x"][t] + 1, c[t]
 
 
 _PINNED = []                                       # the pinned tensors behind the views pinned() hands out
