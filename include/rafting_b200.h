@@ -762,13 +762,16 @@ int rafting_state_digest(rafting_engine_t* e, uint32_t first_gid, uint32_t count
                          uint64_t* digests /* [count], host */);
 int rafting_log_term    (rafting_engine_t* e, uint32_t gid, int64_t index, int64_t* term /* -1 = null */);
 /* in-HBM checkpoint of every table (RaftContext.initialize restores from StableLock + RaftLog; here
-   the whole shard is snapshotted / rolled back at once).  One shadow copy per engine. */
+   the whole shard is snapshotted / rolled back at once).  One shadow copy per engine.  A table created after the
+   checkpoint (the compact path's in-flight table, on its first use) held nothing then: a restore empties it. */
 int rafting_checkpoint(rafting_engine_t* e);
 int rafting_restore   (rafting_engine_t* e);
 int rafting_restore_async(rafting_engine_t* e);   /* the same, enqueued on the step stream without a host synchronisation */
 /* the same state as ONE file that survives the process (planned restart / move of a shard): header + checksummed blocks,
    written to <path>.tmp, fdatasync'ed and renamed.  Load needs an engine created with the same max_groups / replicas; it
-   verifies every block before touching the tables.  Drains the step stream; RAFTING_E_BUSY while a host step is in flight. */
+   verifies every block before touching the tables.  An image saved before the compact path was used carries no in-flight
+   table: loading it empties the engine's; any other difference in the number of tables is RAFTING_E_INVAL.  Drains the
+   step stream; RAFTING_E_BUSY while a host step is in flight. */
 int rafting_state_save(rafting_engine_t* e, const char* path);
 int rafting_state_load(rafting_engine_t* e, const char* path);
 
@@ -908,7 +911,10 @@ int rafting_allgather_join  (rafting_engine_t* e);  /* the step stream waits for
 int rafting_allgather_last  (rafting_engine_t* e, int64_t* host_out /* [world*G] */);  /* the most recently gathered vector */
 /* n device-resident steps enqueued by one call (ins[k] -> outs[k], in order): what a pump thread with a queue of decoded
    batches does, without n trips through the binding.  gather != 0: each step is followed by
-   rafting_allgather_commit_from(outs[k].commit_index). */
+   rafting_allgather_commit_from(outs[k].commit_index), which reads max_groups entries of that column, so every launch must
+   be a whole-shard one (no active list: its commit column is not the [max_groups] end-of-step snapshot), the stream the
+   engine's own, and rafting_comm_init done.  All n launches are checked before any is enqueued: a refused call
+   (RAFTING_E_INVAL, RAFTING_E_CAPACITY for n_active > max_groups, RAFTING_E_NCCL without a communicator) enqueues nothing. */
 int rafting_step_device_seq(rafting_engine_t* e, const rafting_inbox_t* ins_dev, const rafting_outbox_t* outs_dev, uint32_t n,
                             int gather, void* stream);
 

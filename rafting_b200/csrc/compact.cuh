@@ -355,6 +355,10 @@ struct CompactState {
 };
 static void compact_release(rafting_engine* e) { delete e->compact; e->compact = nullptr; }   // the buffers are in dev_allocs
 static uint32_t* compact_bits(rafting_engine* e) { return e->compact ? e->compact->bits : nullptr; }
+// p is one of the in-flight table's three allocations
+static bool compact_owns(const rafting_engine* e, const void* p) {
+    return e->compact && (p == e->compact->table || p == e->compact->tinc || p == e->compact->bits);
+}
 static int compact_state(rafting_engine* e) {
     if (e->compact) return RAFTING_OK;
     CompactState* c = new CompactState();

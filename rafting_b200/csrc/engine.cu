@@ -118,6 +118,7 @@ static void due_release(rafting_engine* e);
 static void edit_release(rafting_engine* e);
 static int compact_state(rafting_engine* e);
 static uint32_t* compact_bits(rafting_engine* e);
+static bool compact_owns(const rafting_engine* e, const void* p);
 static int quiesce_for_table_edit(rafting_engine* e, const char* who);
 extern "C" uint32_t rafting_abi_version(void) { return RAFTING_ABI_VERSION; }
 extern "C" const char* rafting_last_error(void) { return g_err; }
@@ -416,6 +417,16 @@ extern "C" int rafting_step_device_seq(rafting_engine_t* e, const rafting_inbox_
                                        int gather, void* stream) {
     if (!e || !ins || !outs) return fail(RAFTING_E_INVAL, "null argument");
     if (gather && stream && (cudaStream_t)stream != e->stream) return fail(RAFTING_E_INVAL, "gathers follow the engine's own stream");
+    if (gather && !e->gather[0]) return fail(RAFTING_E_NCCL, "communicator not initialised (rafting_comm_init)");
+    // every launch is checked before any is enqueued: a refused call leaves the stream, the tables and the outboxes alone
+    for (uint32_t k = 0; k < n; k++) {
+        const rafting_inbox_t& in = ins[k];
+        if (in.gids && in.n_active > e->G) return fail(RAFTING_E_CAPACITY, "launch %u: n_active > max_groups", k);
+        if ((uint64_t)in.rows * (in.gids ? in.n_active : e->G) * e->F >= (1ull << 32))
+            return fail(RAFTING_E_CAPACITY, "launch %u: rows * groups * followers must stay below 2^32 per step", k);
+        // a gather copies max_groups entries of the launch's commit column: only a whole-shard launch writes all of them
+        if (gather && in.gids) return fail(RAFTING_E_INVAL, "launch %u: a gathering sequence takes whole-shard launches only", k);
+    }
     for (uint32_t k = 0; k < n; k++) {
         // without gathers, launch k's only predecessor on the stream is launch k-1's step kernel: none of them writes an inbox
         e->follows_step = k > 0 && !gather;
@@ -989,13 +1000,17 @@ extern "C" int rafting_checkpoint(rafting_engine_t* e) {
     CU(cudaStreamSynchronize(e->stream));
     return RAFTING_OK;
 }
-// The checkpoint covers the allocations that existed when it was taken (the tables); buffers created later (the
-// gather buffers of rafting_comm_init) are not state and are left alone.
+// The checkpoint copies the state allocations that existed when it was taken (the tables).  A state allocation created
+// later (the compact path's in-flight table, on its first use) held nothing at the checkpoint: a restore zeroes it, so
+// no tag handed out after the checkpoint survives the rollback.  Scratch (the gather buffers of rafting_comm_init,
+// staging) is not state and is left alone.
 static int restore_enqueue(rafting_engine* e) {
     if (e->shadow.empty()) return fail(RAFTING_E_INVAL, "no checkpoint taken");
     CU(cudaSetDevice(e->cfg.device));
     for (size_t i = 0; i < e->shadow.size(); i++)
         if (e->shadow[i]) CU(cudaMemcpyAsync(e->dev_allocs[i], e->shadow[i], e->dev_bytes[i], cudaMemcpyDeviceToDevice, e->stream));
+    for (size_t i = e->shadow.size(); i < e->dev_allocs.size(); i++)
+        if (e->dev_is_state[i]) CU(cudaMemsetAsync(e->dev_allocs[i], 0, e->dev_bytes[i], e->stream));
     return RAFTING_OK;
 }
 extern "C" int rafting_restore(rafting_engine_t* e) {
@@ -1081,11 +1096,18 @@ extern "C" int rafting_state_load(rafting_engine_t* e, const char* path) {
     if (h.version != RAFTING_ABI_VERSION || h.G != e->G || h.F != e->F || h.runs != (uint32_t)KRUNS) {
         close(fd); return fail(RAFTING_E_INVAL, "image of a different shape (G %u F %u runs %u abi %u)", h.G, h.F, h.runs, h.version);
     }
-    // an image taken after the compact path was used carries the in-flight table: create ours before matching blocks
-    std::vector<size_t> ids;
+    // an image taken after the compact path was used carries the in-flight table: create ours before matching blocks.  One
+    // taken before carries none: it is loaded into the other blocks, and our table is zeroed (nothing in flight), as it was
+    // when the image was saved
+    std::vector<size_t> ids, cleared;
     for (size_t i = 0; i < e->dev_allocs.size(); i++) if (e->dev_is_state[i]) ids.push_back(i);
     if (h.nblocks == ids.size() + 3) { rc = compact_state(e); if (rc) { close(fd); return rc; } ids.clear(); for (size_t i = 0; i < e->dev_allocs.size(); i++) if (e->dev_is_state[i]) ids.push_back(i); }
-    if (h.nblocks > ids.size()) { close(fd); return fail(RAFTING_E_INVAL, "image holds %u blocks, the engine %zu", h.nblocks, ids.size()); }
+    if (e->compact && h.nblocks + 3 == ids.size()) {
+        std::vector<size_t> keep;
+        for (size_t i : ids) (compact_owns(e, e->dev_allocs[i]) ? cleared : keep).push_back(i);
+        ids.swap(keep);
+    }
+    if (h.nblocks != ids.size()) { close(fd); return fail(RAFTING_E_INVAL, "image holds %u blocks, the engine %zu", h.nblocks, ids.size()); }
     // read + verify everything first: a corrupt image must not leave the tables half loaded
     std::vector<std::vector<uint8_t>> blocks(h.nblocks);
     for (uint32_t k = 0; k < h.nblocks; k++) {
@@ -1096,6 +1118,8 @@ extern "C" int rafting_state_load(rafting_engine_t* e, const char* path) {
     }
     close(fd);
     for (uint32_t k = 0; k < h.nblocks; k++) CU(cudaMemcpy(e->dev_allocs[ids[k]], blocks[k].data(), blocks[k].size(), cudaMemcpyHostToDevice));
+    for (size_t i : cleared) CU(cudaMemsetAsync(e->dev_allocs[i], 0, e->dev_bytes[i], e->stream));
+    CU(cudaStreamSynchronize(e->stream));
     return RAFTING_OK;
 }
 

@@ -1,6 +1,7 @@
 """rafting_step_device_seq against the CPU oracle: one call enqueues a whole window of device-resident launches, and from
 the second launch on pair_kernel is launched programmatically behind the previous one (it stages its first inbox rows
-before the previous launch has finished).  Every launch's outbox and the end state must be bit-exact.  Needs an H100
+before the previous launch has finished).  Every launch steps into its own poisoned outbox (harness.POISON), so a cell it
+should write and leaves alone differs from the oracle's; every outbox and the end state must be bit-exact.  Needs an H100
 (`-m gpu`)."""
 import numpy as np
 import pytest
@@ -30,12 +31,12 @@ def test_device_sequence_matches_oracle(G, rows, launches):
     ibs, want = [], []
     for k in range(launches):
         ib = workload.leader_inbox_host(w, k, prev)
-        prev = o.step(ib)
+        prev = o.step(ib, out=harness.poisoned_outbox(ib, F, G))
         ibs.append(ib)
         want.append(prev)
     dev = torch.device("cuda", 0)
     dins = [devbatch.DevInbox.from_host(ib, dev) for ib in ibs]
-    douts = [devbatch.DevOutbox(rows, G, F, G, dev) for _ in range(launches)]
+    douts = [devbatch.DevOutbox(rows, G, F, G, dev, fill=harness.POISON) for _ in range(launches)]
     torch.cuda.synchronize()
     ics = (abi.InboxC * launches)(*[d.as_c() for d in dins])
     ocs = (abi.OutboxC * launches)(*[d.as_c() for d in douts])
